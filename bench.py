@@ -1,19 +1,21 @@
 #!/usr/bin/env python
-"""bench.py -- agent-steps/sec of the DecentralPlannerNet hot path on B200.
+"""bench.py -- agent-steps/sec of the DecentralPlannerNet hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one addGSO + forward of one batch of synthetic rollout-like input at the configuration
 BASELINE.json quotes the metric on (configs[1], "C2"): DCP K=3, 10 agents, 20x20 map, batch 64
 inference per GPU (640 agent-steps per step per GPU, weak scaling, no collective on the data path).
 
-How every number is timed: W untimed warm-up steps, then R windows of EXACTLY K back-to-back steps, each
-window bracketed by CUDA events on the launching stream; R is chosen so that the windows cover >= ~100 ms
-(a single 20-step window is 1.2 ms here -- shorter than a host scheduler quantum, which made the 8-rank
-maximum a measure of submission jitter in round 1).  A rank's figure is the MEDIAN window, the reported
-figure the MAX over ranks of that, after a barrier + torch.cuda.synchronize() on both sides.  Inputs rotate
-through a device pool larger than L2.
+How every number is timed: W untimed warm-up steps, then ONE window of exactly K back-to-back steps, bracketed by
+CUDA events on the launching stream (host clock + synchronize for the host-buffer calls).  A step takes tens of
+microseconds, so pass a K that makes the window long against scheduler noise (the default 2000 steps is ~0.1 s).
+The reported figure is the MAX over ranks, after a barrier + torch.cuda.synchronize() on both sides.  Inputs rotate
+through a device pool larger than L2 and are the same from run to run (seeded).
+
+--dump-outputs DIR writes what the timed `value` path returned in its last timed step (the [N, B, 5] float32 logits
+of DecentralPlannerNet.infer_async) as DIR/logits.npy, so that two builds can be compared output for output.
 
 value   C2 device-resident (inputs already in HBM), 6 independent episode batches in flight over the library's compute
         lanes (DecentralPlannerNet.infer_async / join); `single_stream` = the same steps one after the other on one stream.
@@ -26,12 +28,11 @@ legs    the other BASELINE.json configs, same timing rules: C1 (K=2, batch 1, fl
         episodes over 8 GPUs; with N > 1 ranks the flat-gradient NCCL all-reduce runs INSIDE the timed step).
 roofline / roofline_graph_filter / roofline_graph_filter_saturated
         algorithmic flops / bytes per launch (SURVEY.md 8d) over the kernel's mean duration from CUDA events
-        recorded around each kernel on the launching stream; `traffic` = DRAM bytes per launch from the committed
-        ncu captures (profiles/), scaled to this launch's size.
+        recorded around each kernel on the launching stream.
 cpu_baseline   the oracle port (oracle/planner_oracle.py: the reference's own PyTorch-CPU op sequence) on this
         box's host cores, bounded sample of the SAME workload (rank 0, N=1 only).
---impl reference   times that same CPU path as the reference arm (the reference is pure Python/PyTorch and
-        /root/reference does not travel to the GPU box).
+--impl reference   times that same CPU path as the reference arm (the reference is pure Python/PyTorch; the oracle
+        port is its op sequence, shipped with this repository).
 """
 import argparse
 import ctypes as C
@@ -55,13 +56,7 @@ WORKLOAD = "DCP K=3, 10 agents, 20x20 map, batch=64 inference per GPU (BASELINE.
 
 # SURVEY.md section 8d algorithmic figures
 FE_FLOPS_PER_AGENT_STEP = 2476224 + 32768          # 5 conv layers + compress MLP
-# DRAM traffic per unit from the committed ncu captures (dram__bytes_read.sum + dram__bytes_write.sum):
-#   profiles/r02_ncu_feature_mma_c2.csv: feature_mma_kernel per C2 launch (640 agent-steps)
-#   profiles/r02_ncu_gf_small_c2.txt: gf_small_mma_kernel 0.593 MB per C2 launch
-#   profiles/r02_ncu_pair_v16_summary.txt: gf_fwd_pair_kernel 664.54 MB for 65,536 episodes x 10 agents
-NCU_FE_BYTES_PER_AGENT_STEP = 1.752576e6 / 640        # feature_mma_kernel: 0.93 MB of inputs + 0.63 MB of filter images + constants
-NCU_GF_BYTES_PER_AGENT_STEP = 0.593408e6 / 640
-NCU_PAIR_BYTES_PER_AGENT_STEP = 664.54e6 / 655360
+FE_MMA_FROM_AGENTS = 448      # the planner's automatic feature-kernel choice (csrc/planner.cu): wgmma from here, else CUDA cores
 
 
 def gf_bytes_per_agent_step(n):
@@ -77,8 +72,8 @@ def config_dict(world):
     return {"workload": WORKLOAD, "K": K_TAPS, "num_agents": N_AGENTS, "map_w": MAP_W, "batch_per_gpu": BATCH,
             "global_batch": BATCH * world,
             "parallelism": "episode-sharded replicas x%d, no collective on the inference data path" % world,
-            "timing": "median of R windows of K steps (CUDA events), R windows >= ~100 ms, max over ranks",
-            "l2_policy": "device-resident inputs rotate through a pool > 126 MB L2"}
+            "timing": "one window of K steps after W warm-up steps (CUDA events), max over ranks",
+            "l2_policy": "device-resident inputs rotate through a pool > 50 MB L2"}
 
 
 def load_peaks():
@@ -87,7 +82,7 @@ def load_peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), "measured"
     except Exception:
-        return 6650.0, 1400.0, "fallback"       # B200_PROFILING.md fallback figures
+        return 3350.0, 989.0, "H100 SXM data sheet"       # HBM3 GB/s, dense BF16 TFLOP/s (700 W card)
 
 
 class ClockSampler:
@@ -253,11 +248,11 @@ def time_cpu(step, budget_s, min_steps=5, warmup=3):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# timing helper: R windows of K steps
+# timing helper: one window of exactly K steps after W warm-up steps
 # ----------------------------------------------------------------------------------------------------------
 class Timer:
-    def __init__(self, dist, dev, target_ms=100.0, max_windows=400):
-        self.dist, self.dev, self.target_ms, self.max_windows = dist, dev, target_ms, max_windows
+    def __init__(self, dist, dev):
+        self.dist, self.dev = dist, dev
 
     def barrier(self):
         if self.dist is not None:
@@ -265,14 +260,14 @@ class Timer:
         torch.cuda.synchronize()
 
     def device_windows(self, step, K, warmup, drain=None):
-        """step(i) enqueues one step on the current stream (or on the library's lanes: then drain() makes the current
-        stream wait for everything outstanding before a window's closing event).  Returns (median window ms on this
-        rank, windows)."""
+        """step(i) enqueues step i on the current stream (or on the library's lanes: then drain() makes the current
+        stream wait for everything outstanding before the closing event).  Steps 0 .. warmup-1 are untimed, steps
+        warmup .. warmup+K-1 are timed.  Returns (window ms on this rank, windows = 1)."""
         drain = drain or (lambda: None)
         for i in range(warmup):
             step(i)
         drain()
-        torch.cuda.synchronize()
+        self.barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(K):
@@ -280,47 +275,23 @@ class Timer:
         drain()
         e1.record()
         torch.cuda.synchronize()
-        probe = max(e0.elapsed_time(e1), 1e-3)
-        R = int(min(self.max_windows, max(3, round(self.target_ms / probe))))
         self.barrier()
-        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(R)]
-        n = warmup + K
-        for a, b in evs:
-            a.record()
-            for i in range(K):
-                step(n + i)
-            drain()
-            b.record()
-            n += K
-        torch.cuda.synchronize()
-        self.barrier()
-        return float(np.median([a.elapsed_time(b) for a, b in evs])), R
+        return float(e0.elapsed_time(e1)), 1
 
     def host_windows(self, step, K, warmup, drain):
-        """step(i) is a host call (may leave work in flight; drain() completes it).  Wall-clock windows."""
+        """step(i) is a host call (may leave work in flight; drain() completes it).  Wall clock, same step numbering."""
         for i in range(warmup):
             step(i)
         drain()
-        torch.cuda.synchronize()
+        self.barrier()
         t0 = time.perf_counter()
         for i in range(K):
             step(warmup + i)
         drain()
         torch.cuda.synchronize()
-        probe = max((time.perf_counter() - t0) * 1e3, 1e-3)
-        R = int(min(self.max_windows, max(3, round(self.target_ms / probe))))
+        ms = (time.perf_counter() - t0) * 1e3
         self.barrier()
-        times, n = [], warmup + K
-        for _ in range(R):
-            t0 = time.perf_counter()
-            for i in range(K):
-                step(n + i)
-            drain()
-            torch.cuda.synchronize()
-            times.append((time.perf_counter() - t0) * 1e3)
-            n += K
-        self.barrier()
-        return float(np.median(times)), R
+        return ms, 1
 
     def max_over_ranks(self, *vals):
         if self.dist is None:
@@ -383,11 +354,9 @@ def saturated_filter_roofline(gp, dev, batch, hbm_peak, peak_src):
     sec = e0.elapsed_time(e1) * 1e-3 / iters
     nbytes = gf_bytes_per_agent_step(N_AGENTS) * batch * N_AGENTS
     gbs = nbytes / sec / 1e9
-    return {"kernel": "gf_fwd_pair_kernel (tcgen05 cta_group::2, fp16 2-way split, resident taps, TMA tensor stores) via "
+    return {"kernel": "gf_fwd_pair_kernel (wgmma, fp16 2-way split, taps streamed through a bulk-copy ring) via "
                       "gpp_graph_filter_forward",
             "bound": "hbm", "achieved": gbs, "peak": hbm_peak, "unit": "GB/s", "frac": gbs / hbm_peak,
-            "traffic": NCU_PAIR_BYTES_PER_AGENT_STEP * batch * N_AGENTS,
-            "traffic_source": "profiles/r02_ncu_pair_v16_summary.txt (dram read + write at 65,536 episodes, scaled by size)",
             "peak_source": peak_src, "mean_launch_us": sec * 1e6,
             "workload": "K=3, 10 agents, %d episodes (%.0f MB of node signals + GSOs in, %.0f MB out)"
                         % (batch, (batch * N_AGENTS * (128 + N_AGENTS) * 4) / 1e6, batch * N_AGENTS * 128 * 4 / 1e6),
@@ -633,10 +602,12 @@ def main():
     ap.add_argument("--cpu-seconds", type=float, default=10.0)
     ap.add_argument("--pool-mb", type=float, default=160.0, help="device input pool size (> L2)")
     ap.add_argument("--gf-mode", default="auto", choices=["auto", "cuda", "tc", "pair"])
-    ap.add_argument("--fe-mode", default="auto", choices=["auto", "cuda", "tc"])
+    ap.add_argument("--fe-mode", default="auto", choices=["auto", "cuda", "tc", "mma"])
     ap.add_argument("--sat-batch", type=int, default=131072,
                     help="episodes in the saturated graph-filter roofline measurement (0 = skip)")
     ap.add_argument("--no-legs", action="store_true", help="headline configuration only")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the logits of the last timed step of the headline path to DIR/logits.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -648,7 +619,7 @@ def main():
         args.warmup = args.warmup if args.warmup is not None else 3
         run_reference(args, rank, world)
         return
-    args.steps = args.steps if args.steps is not None else 200
+    args.steps = args.steps if args.steps is not None else 2000
     args.warmup = max(3, args.warmup if args.warmup is not None else 20)
     K, W = args.steps, args.warmup
 
@@ -700,6 +671,11 @@ def main():
             while dev_inflight:
                 model.join(dev_inflight.pop(0))
         ms, R = timer.device_windows(dev_async_step, K, W, dev_drain)
+        if args.dump_outputs and rank == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            last = W + K - 1                      # the last timed step wrote its logits into this buffer
+            np.save(os.path.join(args.dump_outputs, "logits.npy"),
+                    dev_outs[last % DEV_DEPTH].float().cpu().numpy())
 
         # ---- per-kernel durations (events recorded around each kernel; PDL is off in this pass) -------
         nat = model._native_for(dev)
@@ -781,10 +757,25 @@ def main():
         fe_s, gf_s = fe_ms.value * 1e-3 / n, gf_ms.value * 1e-3 / n
         fe_tflops = FE_FLOPS_PER_AGENT_STEP * agent_steps / fe_s / 1e12
         gf_gbs = gf_bytes_per_agent_step(N_AGENTS) * agent_steps / gf_s / 1e9
-        sm_mhz = clocks.get("sm_mhz") or clocks.get("sm_max_mhz") or 1965.0
-        fp32_peak = 148 * 128 * 2 * float(sm_mhz) * 1e6 / 1e12
+        sm_mhz = clocks.get("sm_mhz") or clocks.get("sm_max_mhz") or 1980.0
+        fp32_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 128 * 2 * float(sm_mhz) * 1e6 / 1e12
         cfg = config_dict(world)
         cfg["windows"] = R
+        fe_kernel = args.fe_mode if args.fe_mode != "auto" else ("mma" if agent_steps >= FE_MMA_FROM_AGENTS else "cuda")
+        if fe_kernel == "cuda":
+            fe_roofline = {"kernel": "feature_kernel (per-agent CNN + compress MLP on the fp32 CUDA cores)",
+                           "bound": "fp32", "pipe": "FFMA", "peak": fp32_peak,
+                           "peak_source": "SM count x 128 FMA/clk x 2 x sampled SM clock"}
+        else:
+            fe_roofline = {"kernel": {"mma": "feature_mma_kernel (per-agent CNN + compress MLP on wgmma: fp16 2-way split "
+                                             "operands, 3 products per term, fp32 register accumulators)",
+                                      "tc": "feature_tc_kernel (3xTF32 implicit GEMM on wgmma)"}[fe_kernel],
+                           "bound": "tensor", "pipe": "wgmma.mma_async (SASS HGMMA), M=64 per warpgroup",
+                           "peak": tf_peak, "peak_source": peak_src + " bf16 dense",
+                           "note": "the issued tensor work is 3x the algorithmic flops (split products)"}
+        fe_roofline.update({"achieved": fe_tflops, "unit": "TFLOP/s", "frac": fe_tflops / fe_roofline["peak"],
+                            "mean_launch_us": fe_s * 1e6,
+                            "algorithmic_flops_per_launch": FE_FLOPS_PER_AGENT_STEP * agent_steps})
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K,
             "warmup": W, "ms_per_step": ms / K, "higher_is_better": True,
@@ -808,24 +799,12 @@ def main():
                     "sync_api": "DecentralPlannerNet.infer_host -> gpp_planner_forward_host, one blocking call per step"},
             "gpu_launches": int(launches_per_window) * R, "gpu_launches_per_step": int(launches_per_window) / K,
             "clocks": clocks,
-            "roofline": {"kernel": "feature_mma_kernel (per-agent CNN + compress MLP on tcgen05: fp16 2-way split operands, "
-                                   "3 products per term, fp32 accumulation in TMEM -- the dominant kernel of the step by time)",
-                         "bound": "tensor", "pipe": "tcgen05.mma kind::f16 (SASS UTCHMMA), M=128 tiles, 8 agents per CTA",
-                         "achieved": fe_tflops, "peak": tf_peak, "unit": "TFLOP/s", "frac": fe_tflops / tf_peak,
-                         "traffic": NCU_FE_BYTES_PER_AGENT_STEP * agent_steps,
-                         "traffic_source": "profiles/r02_ncu_feature_mma_c2.csv (dram read + write per launch)",
-                         "peak_source": peak_src + " bf16 dense (sustained)",
-                         "mean_launch_us": fe_s * 1e6,
-                         "algorithmic_flops_per_launch": FE_FLOPS_PER_AGENT_STEP * agent_steps,
-                         "note": "640 agents = 80 tiles of 8 on 80 of 148 SMs, one tile per CTA: the launch is latency-bound "
-                                 "(12 serialized MMA / epilogue phases per tile); the issued tensor work is 3x the algorithmic "
-                                 "flops (split products) on M tiles that are 25-60 % padding"},
-            "roofline_graph_filter": {"kernel": "gf_small_mma_kernel (K-tap filter + ReLU + action MLP on tcgen05, clusters "
+            "roofline": fe_roofline,
+            "roofline_graph_filter": {"kernel": "gf_small_mma_kernel (K-tap filter + ReLU + action MLP on wgmma, clusters "
                                                 "of 2 CTAs per 6 episodes; the benchmark size is launch-latency bound: 0.68 MB "
                                                 "per launch)", "bound": "hbm",
                                       "achieved": gf_gbs, "peak": hbm_peak, "unit": "GB/s",
-                                      "frac": gf_gbs / hbm_peak, "traffic": NCU_GF_BYTES_PER_AGENT_STEP * agent_steps,
-                                      "traffic_source": "profiles/r02_ncu_gf_small_c2.txt",
+                                      "frac": gf_gbs / hbm_peak,
                                       "peak_source": peak_src, "mean_launch_us": gf_s * 1e6,
                                       "algorithmic_bytes_per_launch": gf_bytes_per_agent_step(N_AGENTS) * agent_steps,
                                       "algorithmic_flops_per_launch": gf_flops_per_agent_step(N_AGENTS, K_TAPS) * agent_steps},

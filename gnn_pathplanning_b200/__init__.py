@@ -1,4 +1,4 @@
-"""gnn_pathplanning_b200 -- B200 (sm_100a) implementation of the DecentralPlannerNet
+"""gnn_pathplanning_b200 -- H100 (sm_90a) implementation of the DecentralPlannerNet
 forward path of proroklab/gnn_pathplanning behind the reference's own module API.
 
     from gnn_pathplanning_b200 import DecentralPlannerNet, GraphFilterBatch, BatchLSIGF

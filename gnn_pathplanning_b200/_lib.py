@@ -20,7 +20,7 @@ INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include", "gnnpp_b200.h")
 INCLUDE_DEBUG = os.path.join(os.path.dirname(PKG_DIR), "include", "gnnpp_b200_debug.h")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -92,7 +92,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compiles the CUDA sources for sm_100a into the in-tree shared library: one nvcc -c per
+    """Compiles the CUDA sources for sm_90a into the in-tree shared library: one nvcc -c per
     translation unit (in parallel, only the stale ones), then one link."""
     if not force and not _stale():
         return LIB_PATH
@@ -116,7 +116,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
     if verbose:
         print(" ".join(cmd))
     r = subprocess.run(cmd, capture_output=True, text=True)
@@ -140,7 +140,7 @@ def load():
         if not os.path.isfile(LIB_PATH):
             raise RuntimeError(
                 "gnn_pathplanning_b200: %s is missing -- build it with "
-                "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+                "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                 "There is no CPU fallback for this package." % LIB_PATH)
         lib = C.CDLL(LIB_PATH)
         vp, i, sz = C.c_void_p, C.c_int, C.c_size_t

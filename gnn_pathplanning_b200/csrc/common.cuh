@@ -1,4 +1,4 @@
-// Shared helpers for libgnnpp_b200 (sm_100a only).
+// Shared helpers for libgnnpp_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -78,7 +78,7 @@ inline cudaError_t launch_maybe_pdl(Kernel kernel, int grid, int block, size_t s
     return cudaLaunchKernelEx(&cfg, kernel, args);
 }
 
-// ---- device-side PTX helpers (Blackwell: mbarrier + 1-D bulk async copy = UBLKCP) -----
+// ---- device-side PTX helpers (mbarrier + 1-D bulk async copy, sm_90) -----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -133,36 +133,22 @@ __device__ __forceinline__ float4 ld_smem4(const float* p) {
     return *reinterpret_cast<const float4*>(p);
 }
 
-// ---- packed fp32 arithmetic (sm_100: SASS FFMA2 / FMUL2 / FADD2).  One instruction = one issue slot for two IEEE fp32
-//      operations with the rounding of the scalar forms, so results are bit-identical; a scalar factor is broadcast by
-//      the instruction itself (operand modifier .F32), no extra move.  The fp32 pipe's rate is unchanged (128 FMA / clk /
-//      SM, profiles/probes/ffma2_probe.cu): this halves ISSUE pressure where FMAs compete with loads, conversions and
-//      stores for the scheduler. ------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long f2_pack(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void f2_unpack(unsigned long long v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
+// ---- paired fp32 arithmetic on two lanes of data with one scalar factor.  sm_90 has no packed fp32 instruction, so
+//      these are two IEEE operations each (round to nearest, no contraction beyond the explicit fma). --------------
 // (c0, c1) = s * (b0, b1) + (c0, c1)
 __device__ __forceinline__ void ffma2_s(float s, float b0, float b1, float& c0, float& c1) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(f2_pack(s, s)), "l"(f2_pack(b0, b1)), "l"(f2_pack(c0, c1)));
-    f2_unpack(d, c0, c1);
+    c0 = __fmaf_rn(s, b0, c0);
+    c1 = __fmaf_rn(s, b1, c1);
 }
 // (c0, c1) = s * (b0, b1)
 __device__ __forceinline__ void fmul2_s(float s, float b0, float b1, float& c0, float& c1) {
-    unsigned long long d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_pack(s, s)), "l"(f2_pack(b0, b1)));
-    f2_unpack(d, c0, c1);
+    c0 = __fmul_rn(s, b0);
+    c1 = __fmul_rn(s, b1);
 }
 // (c0, c1) = (a0, a1) - (b0, b1)
 __device__ __forceinline__ void fsub2(float a0, float a1, float b0, float b1, float& c0, float& c1) {
-    unsigned long long d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_pack(a0, a1)), "l"(f2_pack(b0, b1)));
-    f2_unpack(d, c0, c1);
+    c0 = __fsub_rn(a0, b0);
+    c1 = __fsub_rn(a1, b1);
 }
 
 }  // namespace gpp

@@ -1,8 +1,8 @@
-// Feature extractor for sm_100a: per-agent CNN (5 x conv3x3+BN+ReLU, 3 max-pools) + compress
+// Feature extractor for sm_90a: per-agent CNN (5 x conv3x3+BN+ReLU, 3 max-pools) + compress
 // MLP, all B*N agents tiled up to 8 at a time onto persistent 16-warp CTAs.
 //
 // Replaces the N sequential per-agent ConvLayers/compressMLP calls of
-// DecentralPlannerNet.forward (/root/reference/graphs/models/decentralplanner.py:284-290) in
+// DecentralPlannerNet.forward (gnn_pathplanning/graphs/models/decentralplanner.py:284-290) in
 // eval mode.  Activations never leave shared memory between layers.
 //
 // Mapping (fp32 FMA).  Shared memory delivers 4 B per lane per clock to the register file, the FMA
@@ -76,10 +76,8 @@ __device__ __forceinline__ float quad_sum(float v) {
 //   MLP  : 4 chunks, 8 inputs of each quarter of the input range          (4 x 4 KB)
 // Every thread tracks the (uniform) counters; thread 0 issues the copy that refills a slot right after the CTA-wide
 // barrier that retires its chunk, three chunks ahead of the consumers.
-// Measured and not kept (profiles/README.md): a cluster-multicast stream (one L2 read per 2 or 4 CTAs, 20 % slower
-// at every batch size) and a 10-slot stream that parks the conv3 / conv4 / MLP filters in the dead ACT1 / ACT2
-// buffers while conv2 computes, with or without per-chunk CTA barriers (15-25 % slower: the extra bookkeeping per
-// chunk costs more than the deeper prefetch returns).
+// Measured (on the previous target GPU) and not kept: a cluster-multicast stream (one L2 read per 2 or 4 CTAs) and a
+// 10-slot stream that parks the conv3 / conv4 / MLP filters in the dead ACT1 / ACT2 buffers while conv2 computes.
 // ---------------------------------------------------------------------------------------------------
 struct WStream {
     float* ring;
@@ -293,7 +291,7 @@ __global__ void __launch_bounds__(FE_THREADS, 1) feature_kernel(const FeArgs A) 
                 const int yy = p / 12 - 1, xx = p % 12 - 1;
                 float v = 0.f;
                 if (a < na && yy >= 0 && yy < 11 && xx >= 0 && xx < 11)
-                    v = __ldg(xg + a * IN_PIX + c * 121 + yy * 11 + xx);
+                    v = __ldcg(xg + a * IN_PIX + c * 121 + yy * 11 + xx);
                 in0[i] = v;
             }
         }

@@ -1,15 +1,15 @@
-// im2col-free tensor-core feature extractor for sm_100a: the per-agent CNN + compress MLP of DecentralPlannerNet
-// (/root/reference/graphs/models/decentralplanner.py:155-195,284-290, eval mode) on tcgen05 with fp16 2-way split
-// operands (fp32 parity), 8 agents per tile, one persistent CTA per SM.
+// im2col-free tensor-core feature extractor (Hopper wgmma): the per-agent CNN + compress MLP of DecentralPlannerNet
+// (reference graphs/models/decentralplanner.py:155-195,284-290, eval mode) with fp16 2-way split operands (fp32
+// parity), 8 agents per tile, one persistent CTA per SM.
 //
 // Layout idea.  An activation map lives in shared memory as fp16 (hi | lo) planes of 8 channels, one 16-byte vector per
 // padded pixel, pixels in ONE linear order over the whole tile:   row = y * (8 agents * Wp) + agent * Wp + x.
-// That is exactly the canonical NO-SWIZZLE K-major UMMA operand layout (rows 16 B apart, 8-row groups 128 B apart,
-// K planes `rows * 16` B apart), and in it the 3x3 tap (ky, kx) of EVERY output pixel is the same buffer shifted by
-// (ky * 8 * Wp + kx) rows: the A operand of a tap is just the descriptor start address moved by a multiple of 16 B
-// (profiles/probes/umma_nosw_probe.cu checks this addressing on the hardware).  No im2col copy exists anywhere: an
-// epilogue writes a layer's output once, and the next layer's 9 taps x Cin/16 MMAs read it in place.  With the
-// y-major order the rows a layer needs (y < Hout) are a prefix, so M covers needed image rows only.
+// That is exactly the canonical NO-SWIZZLE K-major operand layout of a wgmma descriptor (rows 16 B apart, 8-row groups
+// 128 B apart, K planes `rows * 16` B apart), and in it the 3x3 tap (ky, kx) of EVERY output pixel is the same buffer
+// shifted by (ky * 8 * Wp + kx) rows: the A operand of a tap is just the descriptor start address moved by a multiple
+// of 16 B.  No im2col copy exists anywhere: an epilogue writes a layer's output once, and the next layer's 9 taps x
+// Cin/16 MMAs read it in place.  With the y-major order the rows a layer needs (y < Hout) are a prefix, so M covers
+// needed image rows only.
 //
 //   layer  in grid (Hp x Wp)  rows   planes  out ch  M tiles  taps x k16   B bytes
 //   conv0  13 x 16 (11+pad)   1664   1       32      10       3 x 2 (*)    6 KB    (*) two ky taps per K=16: LBO = one row;
@@ -21,13 +21,14 @@
 //   linear 1 x 1              8      16      128     1        1 x 8        64 KB
 //
 // Precision: v = hi + lo with hi = fp16(v * 2^e), lo = fp16(v * 2^e - hi); products hi*hi + lo*hi + hi*lo accumulate
-// in fp32 (TMEM).  e is chosen per agent and layer from the running maximum (two-pass epilogue), weights are scaled per
-// layer; residual ~2^-22 per product.  For N <= 64 the filter operand is [W_hi | W_lo] side by side, so A_hi needs one
-// MMA of width 2N (M=128 MMAs cost ~47-65 cycles whatever N <= 128 is: the A read bounds them) and the two halves of
-// the accumulator are added in the epilogue.
+// in one fp32 register accumulator.  e is chosen per agent and layer from the running maximum (two-pass epilogue),
+// weights are scaled per layer; residual ~2^-22 per product.  For N <= 64 the filter image holds [W_hi | W_lo] side
+// by side (2N rows per K plane); for N = 128 the two are separate 128-row planes.
 //
-// Roles: warp 0 = MMA issuer, warp 1 = loader (filter chunks through a 5 x 16 KB ring of bulk copies, input tiles),
-// warps 2-9 = epilogue (TMEM -> BatchNorm/ReLU/max-pool -> fp16 split -> next layer's operand buffer).
+// Roles: warps 0-7 = two warpgroups, one per half of the output channels: each issues the wgmma of its channels for
+// all rows (M = 64 per instruction), stages its accumulators through shared memory and runs the epilogue
+// (BatchNorm/ReLU/max-pool -> fp16 split -> next layer's operand buffer); warp 8 = loader (filter chunks through a
+// 5 x 16 KB ring of bulk copies, input tiles).
 #include "common.cuh"
 #include "feature.cuh"
 #include "tc_common.cuh"
@@ -40,7 +41,8 @@ namespace gpp {
 constexpr int FM_A = 8;                        // agents per tile
 constexpr int FM_EPI_WARPS = 8;
 constexpr int FM_EPI_THREADS = 32 * FM_EPI_WARPS;
-constexpr int FM_THREADS = 64 + FM_EPI_THREADS;
+constexpr int FM_LOADER_WARP = FM_EPI_WARPS;
+constexpr int FM_THREADS = FM_EPI_THREADS + 32;
 constexpr int FM_SLOTS = 5, FM_SLOT_BYTES = 16384;
 constexpr int FM_NL = 6;
 
@@ -82,10 +84,8 @@ __host__ __device__ constexpr int fm_in_base(int L) { return (L == 0 || L == 2 |
 
 struct FmMisc {
     uint64_t w_full[FM_SLOTS], w_free[FM_SLOTS];
-    uint64_t acc0_full[2], acc0_free[2];
-    uint64_t layer_full, act_ready, xraw_full, xraw_free;
-    uint32_t tmem_slot;
-    uint32_t xflag[2];                 // tile has a non-zero lo part in its inputs
+    uint64_t xraw_full, xraw_free;
+    uint32_t xflag;                    // tile has a non-zero lo part in its inputs
     uint32_t amax[FM_NL][FM_A];        // running max (float bits, values >= 0) of layer L's output per agent
     float mul0[FM_A], inv0[FM_A];      // input scale 2^e0 and its inverse
     float mul1[FM_A], inv1[FM_A];      // act1 scale (from the weight-norm bound of conv0) and its inverse
@@ -109,11 +109,6 @@ struct FmArgs {
 
 // ---- waits -------------------------------------------------------------------------------------------------------
 constexpr long long FM_WATCHDOG_CYCLES = 2000000000LL;
-__device__ __noinline__ void fm_watchdog_trap(int id, uint32_t parity) {
-    printf("feature_mma_kernel: watchdog -- block %d warp %d stuck on barrier %d parity %u\n", (int)blockIdx.x,
-           (int)(threadIdx.x >> 5), id, parity);
-    __trap();
-}
 __device__ __forceinline__ bool fm_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -125,15 +120,13 @@ __device__ __forceinline__ bool fm_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ void fm_wait(uint64_t* bar, uint32_t parity, int id) {
+// Watchdog: a barrier that does not complete within ~1 s traps instead of hanging the GPU.  No printf: a function call
+// anywhere in the kernel makes ptxas serialise its wgmma pipelines.
+__device__ __forceinline__ void fm_wait(uint64_t* bar, uint32_t parity) {
     if (fm_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!fm_try_wait(bar, parity))
-        if (clock64() - t0 > FM_WATCHDOG_CYCLES) fm_watchdog_trap(id, parity);
-}
-__device__ __forceinline__ void fm_wait_warp(uint64_t* bar, uint32_t parity, int id) {
-    if ((threadIdx.x & 31) == 0) fm_wait(bar, parity, id);
-    __syncwarp();
+        if (clock64() - t0 > FM_WATCHDOG_CYCLES) __trap();
 }
 __device__ __forceinline__ void fm_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -143,40 +136,6 @@ __device__ __forceinline__ void fm_arrive_warp(uint64_t* bar) {
     if ((threadIdx.x & 31) == 0) fm_arrive(bar);
 }
 __device__ __forceinline__ void fm_epi_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// ---- UMMA helpers (no-swizzle K-major descriptors, kind::f16) --------------------------------------------------------
-__device__ __forceinline__ uint64_t fm_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
-}
-// Issued from an `if (lane == 0)` region the compiler wraps every tcgen05.mma in a lane loop (ELECT / R2UR.BROADCAST /
-// BRA.U.ANY), ~50 cycles per instruction -- about the 47-65 cycles the tensor pipe needs for an M=128 MMA, so the pipe
-// stays busy.  A PREDICATED second MMA doubles that (the loop runs whether or not the predicate holds), which is why
-// conv0 has two separate code paths; electing a lane per instruction with all lanes running the loops (CUTLASS' way)
-// measured slower here: ~70 cycles per MMA (profiles/r02_fm_phase_timing.txt).
-__device__ __forceinline__ void fm_commit(uint64_t* bar) { umma_commit(bar); }
-__device__ __forceinline__ void fm_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void fm_tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void fm_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // scale exponent for a running maximum m >= 0 (float bits): m * 2^e in [2^9, 2^10)
 __device__ __forceinline__ int fm_scale_exp(uint32_t bits) {
@@ -204,102 +163,84 @@ __device__ __forceinline__ void fm_sts16(uint32_t addr, const uint4 v) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
-// debug phase timers (A.timing != null): slots 0-5 MMA wait-for-input per layer, 6-11 MMA wait-for-filters, 12-17 MMA issue,
-// 18 tiles, 19 convert, 20-25 epilogue wait-for-accumulator per layer, 26-31 epilogue work per layer (warp 2 of block 0)
-#define FM_T0() const long long _t0 = timing ? clock64() : 0
-#define FM_ACC(slot) do { if (timing) tacc[slot] += (unsigned long long)(clock64() - _t0); } while (0)
+// debug phase timers (A.timing != null): 6-11 wait-for-filters per layer, 12-17 MMA per layer, 18 tiles, 19 convert,
+// 26-31 epilogue work per layer (warp 0 of block 0)
+// tacc = the debug buffer in the one thread that records (thread 0 of block 0), null everywhere else
+#define FM_T0() const long long _t0 = tacc ? clock64() : 0
+#define FM_ACC(slot) do { if (tacc) atomicAdd(&tacc[slot], (unsigned long long)(clock64() - _t0)); } while (0)
 
-// ---- MMA issue of one layer (L >= 1) -------------------------------------------------------------------------------
-// Everything but the ring slot is a compile-time constant: the loops are fully unrolled and a descriptor is one 32-bit
-// add on its low word (address field; smem addresses < 256 KB never carry into the LBO field at bit 16).  A looped
-// version that rebuilt the descriptors per instruction spent ~75-85 cycles per MMA in address arithmetic on the single
-// issuing thread (profiles/r02_fm_phase_v1.txt) -- longer than the 47-65 cycles the tensor pipe needs for it.
-constexpr uint32_t FM_DESC_HI = (128u >> 4) | (1u << 14);      // SBO = 128 B, descriptor version 1
-__device__ __forceinline__ uint64_t fm_desc_w(uint32_t lo) { return ((uint64_t)FM_DESC_HI << 32) | lo; }
-__host__ __device__ constexpr uint32_t fm_lbo_field(uint32_t lbo) { return ((lbo >> 4) & 0x3FFF) << 16; }
-
-struct FmIssue {
-    uint32_t sm16;        // shared-memory base >> 4
-    uint32_t tmem;
-    uint32_t slot, phase; // ring position of the next chunk
+// ring position of the next filter chunk (the same sequence the loader fills)
+struct FmRing {
+    uint32_t slot, phase;
+    __device__ __forceinline__ void advance() { if (++slot == FM_SLOTS) { slot = 0; phase ^= 1; } }
 };
+__device__ __forceinline__ uint64_t fm_desc(uint32_t addr, uint32_t lbo) { return gmma_desc_nosw(addr, lbo, 128); }
 
-template <int L, int CC>
-__device__ __forceinline__ void fm_issue_chunks(FmIssue& is, FmMisc* ms, bool timing, unsigned long long* tacc) {
-    if constexpr (CC < fm_chunks(L)) {
-        constexpr int N = fm_n(L), KS = fm_ks(L), UNITS = fm_units(L), UPC = fm_upc(L), UB = fm_unit_bytes(L);
-        constexpr int AW = fm_aw(L), LBO = (L == 5) ? 128 : fm_lbo(L), TILES = fm_tiles(L);
-        constexpr uint32_t A_HI = fm_in_base(L), A_LO = fm_in_base(L) + fm_planes(L) * LBO;
-        constexpr int DCOLS = (L <= 3) ? 2 * N : N;
-        constexpr int NU = (UNITS - CC * UPC) < UPC ? (UNITS - CC * UPC) : UPC;
+// ---- MMAs of one layer L >= 1 for this warpgroup's half h of the output channels: acc[t][mh] = rows t * 128 + 64 mh ..
+//      of the layer's M tiles, N / 2 channels.  Every descriptor offset is a compile-time constant (fully unrolled).
+template <int L>
+__device__ __forceinline__ constexpr int fm_mh() { return L >= 3 ? 1 : 2; }     // conv3 / conv4 / linear: rows < 64 only
+
+template <int L, typename Acc>
+__device__ __forceinline__ void fm_mma_layer(uint32_t sm_base, FmMisc* ms, FmRing& ring, int h, Acc& acc, unsigned long long* tacc) {
+    constexpr int N = fm_n(L), NW = N / 2, KS = fm_ks(L), UNITS = fm_units(L), UPC = fm_upc(L), UB = fm_unit_bytes(L);
+    constexpr int AW = fm_aw(L), LBO = (L == 5) ? 128 : fm_lbo(L), TILES = fm_tiles(L), MH = fm_mh<L>();
+    constexpr uint32_t A_HI = fm_in_base(L), A_LO = fm_in_base(L) + fm_planes(L) * LBO;
+    constexpr int CHUNKS = fm_chunks(L);
+    // B rows of this channel half: [W_hi | W_lo] planes of 2N rows (N <= 64), or separate 128-row W_hi / W_lo planes
+    const uint32_t b_hi_off = (L <= 3) ? (uint32_t)(h * NW * 16) : (uint32_t)(h * 64 * 16);
+    const uint32_t b_lo_off = (L <= 3) ? (uint32_t)((N + h * NW) * 16) : (uint32_t)(4096 + h * 64 * 16);
+    constexpr uint32_t BLBO = (L <= 3) ? 32 * N : 2048;
+#pragma unroll
+    for (int cc = 0; cc < CHUNKS; ++cc) {
         {
             FM_T0();
-            fm_wait(&ms->w_full[is.slot], is.phase, 10 + is.slot);
+            fm_wait(&ms->w_full[ring.slot], ring.phase);
             FM_ACC(6 + L);
         }
-        tcgen05_fence_after();
         FM_T0();
-        const uint32_t a_hi = is.sm16 + (A_HI >> 4) + fm_lbo_field(LBO), a_lo = is.sm16 + (A_LO >> 4) + fm_lbo_field(LBO);
-        const uint32_t bs = is.sm16 + ((FM_RING + is.slot * FM_SLOT_BYTES) >> 4) + fm_lbo_field(L <= 3 ? 32 * N : 2048);
+        const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES;
+        wgmma_fence();
 #pragma unroll
-        for (int uu = 0; uu < NU; ++uu) {
-            const int u = CC * UPC + uu;
-            const int tap = u / KS, k16 = u - tap * KS;
-            const int shift = (L == 5) ? 0 : ((tap / 3) * AW + (tap % 3));
+        for (int uu = 0; uu < UPC; ++uu) {
+            const int u = cc * UPC + uu;
+            if (u < UNITS) {
+                const int tap = u / KS, k16 = u - tap * KS;
+                const int shift = (L == 5) ? 0 : ((tap / 3) * AW + (tap % 3));
+                const uint64_t db_hi = fm_desc(bs + uu * UB + b_hi_off, BLBO), db_lo = fm_desc(bs + uu * UB + b_lo_off, BLBO);
 #pragma unroll
-            for (int t = 0; t < TILES; ++t) {
-                const uint32_t aoff = (uint32_t)(((t * 128 + shift) * 16 + k16 * 2 * LBO) >> 4);
-                const uint32_t d = is.tmem + t * DCOLS;
-                if (L <= 3) {
-                    const uint64_t db = fm_desc_w(bs + ((uu * UB) >> 4));     // planes of [W_hi | W_lo]: 2N rows of 16 B
-                    fm_mma(d, fm_desc_w(a_hi + aoff), db, umma_idesc_f16(128, 2 * N), u > 0);
-                    fm_mma(d, fm_desc_w(a_lo + aoff), db, umma_idesc_f16(128, N), 1);
-                } else {
-                    const uint64_t db_hi = fm_desc_w(bs + ((uu * UB) >> 4)), db_lo = fm_desc_w(bs + ((uu * UB + 4096) >> 4));
-                    fm_mma(d, fm_desc_w(a_hi + aoff), db_hi, umma_idesc_f16(128, 128), u > 0);
-                    fm_mma(d, fm_desc_w(a_lo + aoff), db_hi, umma_idesc_f16(128, 128), 1);
-                    fm_mma(d, fm_desc_w(a_hi + aoff), db_lo, umma_idesc_f16(128, 128), 1);
-                }
+                for (int t = 0; t < TILES; ++t)
+#pragma unroll
+                    for (int mh = 0; mh < MH; ++mh) {
+                        const uint32_t aoff = (uint32_t)((t * 128 + mh * 64 + shift) * 16 + k16 * 2 * LBO);
+                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_HI + aoff, LBO), db_hi, u > 0);
+                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_LO + aoff, LBO), db_hi, 1);
+                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_HI + aoff, LBO), db_lo, 1);
+                    }
             }
         }
-        fm_commit(&ms->w_free[is.slot]);
-        if (++is.slot == FM_SLOTS) { is.slot = 0; is.phase ^= 1; }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fm_arrive_warp(&ms->w_free[ring.slot]);
+        ring.advance();
         FM_ACC(12 + L);
-        fm_issue_chunks<L, CC + 1>(is, ms, timing, tacc);
     }
-}
-template <int L>
-__device__ __forceinline__ void fm_issue_layer(FmIssue& is, FmMisc* ms, bool timing, unsigned long long* tacc) {
-    fm_issue_chunks<L, 0>(is, ms, timing, tacc);
-    fm_commit(&ms->layer_full);
 }
 
 // ---- epilogue pieces -----------------------------------------------------------------------------------------------
 __device__ __forceinline__ float4 fm_lds4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
-// 16 output channels of this thread's accumulator row: (acc (+ the [.. | W_lo] half)) * (scale * inv) + shift, ReLU.
-// taddr = TMEM address of the first column, cs = shared-memory constants of the first channel ([0..] scale, [128..] shift)
-template <int L>
-__device__ __forceinline__ void fm_block_vals(uint32_t taddr, const float* cs, float inv, float (&u)[16]) {
-    constexpr int N = fm_n(L);
-    float a[16];
-    fm_tmem_ld16(taddr, a);
-    if (L <= 3) {
-        float b[16];
-        fm_tmem_ld16(taddr + N, b);
-        fm_tmem_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) a[i] += b[i];
-    } else {
-        fm_tmem_wait_ld();
-    }
+// 16 output channels of this thread's accumulator row: acc * (scale * inv) + shift, ReLU.  src = the staged accumulator
+// of the first channel, cs = shared-memory constants of the first channel ([0..] scale, [128..] shift)
+__device__ __forceinline__ void fm_block_vals(const float* src, const float* cs, float inv, float (&u)[16]) {
 #pragma unroll
     for (int i = 0; i < 16; i += 4) {
+        const float4 a = fm_lds4(src + i);
         const float4 sc = fm_lds4(cs + i), sh = fm_lds4(cs + 128 + i);
-        u[i] = fmaxf(fmaf(a[i], sc.x * inv, sh.x), 0.f);
-        u[i + 1] = fmaxf(fmaf(a[i + 1], sc.y * inv, sh.y), 0.f);
-        u[i + 2] = fmaxf(fmaf(a[i + 2], sc.z * inv, sh.z), 0.f);
-        u[i + 3] = fmaxf(fmaf(a[i + 3], sc.w * inv, sh.w), 0.f);
+        u[i] = fmaxf(fmaf(a.x, sc.x * inv, sh.x), 0.f);
+        u[i + 1] = fmaxf(fmaf(a.y, sc.y * inv, sh.y), 0.f);
+        u[i + 2] = fmaxf(fmaf(a.z, sc.z * inv, sh.z), 0.f);
+        u[i + 3] = fmaxf(fmaf(a.w, sc.w * inv, sh.w), 0.f);
     }
 }
 __device__ __forceinline__ float fm_max16(const float (&u)[16]) {
@@ -336,38 +277,48 @@ __device__ __forceinline__ void fm_zero(uint32_t addr, int bytes, int et) {
     for (int i = et * 16; i < bytes; i += FM_EPI_THREADS * 16) fm_sts16(addr + i, z);
 }
 
-// dynamic-scale layers 1..4: zero the target buffer, wait for the accumulators, pass 1 = values (kept in registers) +
-// per-agent maximum (+ pooling partners that live in another warp go through FM_STG), pass 2 = scale, split, store
+// row stride (floats) of an accumulator tile staged in shared memory: padded against bank conflicts of row-per-lane reads
+__host__ __device__ constexpr int fm_srow(int L) { return fm_n(L) + 4; }
+
+// layers 1..5: MMAs into registers; per M tile the accumulators are staged (rows x fm_srow floats) in the layer's INPUT
+// buffer, which no MMA reads any more.  Dynamic-scale layers 1..4 then run pass 1 = values (kept in registers) +
+// per-agent maximum (+ pooling partners that live in another warp go through FM_STG), pass 2 = scale, split, store.
 template <int L>
-__device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_base, uint32_t tmem_lane, FmMisc* ms, int na,
-                                                int q, int h, int lane, int et, uint32_t& gl, bool timing,
-                                                unsigned long long* tacc) {
-    constexpr int N = fm_n(L), AW = fm_aw(L), WP = fm_wp(L), HO = fm_hout(L), TILES = fm_tiles(L);
-    constexpr int DCOLS = (L <= 3) ? 2 * N : N;
+__device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_base, FmMisc* ms, FmRing& ring, int na,
+                                                int q, int h, int lane, int et, unsigned long long* tacc) {
+    constexpr int N = fm_n(L), AW = fm_aw(L), WP = fm_wp(L), HO = fm_hout(L), TILES = fm_tiles(L), MH = fm_mh<L>();
     constexpr bool POOL = (L == 2 || L == 4);
     constexpr int LO = L + 1;                                      // the layer that consumes the output
     constexpr uint32_t OUT = fm_in_base(LO);
     constexpr int OLBO = (LO == 5) ? 128 : fm_lbo(LO), OPL = fm_planes(LO), OAW = fm_aw(LO), OWP = fm_wp(LO);
     constexpr int NB = N / 32;                                     // 16-channel blocks per thread (channel half h)
     constexpr int CV = POOL ? 8 : 16;
-    fm_zero(sm_base + OUT, (LO == 5) ? 8192 : 2 * OPL * OLBO, et);
-    {
-        FM_T0();
-        fm_wait_warp(&ms->layer_full, gl & 1, 30 + L);
-        FM_ACC(20 + L);
-    }
-    ++gl;
-    tcgen05_fence_after();
+    constexpr int SROW = fm_srow(L);
+    const int wt = et & 127;                                       // thread of the warpgroup
+    float acc[TILES][MH][N / 4];
+    fm_mma_layer<L>(sm_base, ms, ring, h, acc, tacc);
+    fm_epi_sync();                                                 // both warpgroups' MMAs are done with the input buffer
     FM_T0();
+    fm_zero(sm_base + OUT, (LO == 5) ? 8192 : 2 * OPL * OLBO, et);
+    float* sacc = reinterpret_cast<float*>(sm + fm_in_base(L));
     float* stg = reinterpret_cast<float*>(sm + FM_STG);
     const float* cs = reinterpret_cast<const float*>(sm + FM_CST) + L * 256 + h * (N / 2);
     const int l = q * 32 + lane, odd = lane & 1;
     const bool rows_here = (L == 1 || L == 2) ? true : (q < 2);     // conv3 / conv4: the valid rows are lanes 0..63
     const bool upper = (L == 2) ? (q >= 2) : (q == 1);              // pooled layers: rows whose y is odd
     float cv[TILES][NB][CV];
-    if (rows_here) {
 #pragma unroll
-        for (int t = 0; t < TILES; ++t) {
+    for (int t = 0; t < TILES; ++t) {
+        if (t > 0) fm_epi_sync();                                   // pass 1 of tile t - 1 has read the staging buffer
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh)
+#pragma unroll
+            for (int i = 0; i < N / 4; i += 2) {
+                const int row = 64 * mh + wg_row(wt, i), col = h * (N / 2) + wg_col(wt, i);
+                *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[t][mh][i], acc[t][mh][i + 1]);
+            }
+        fm_epi_sync();
+        if (rows_here) {
             const int r = t * 128 + l;
             const int y = r / AW, a = (r % AW) / WP, x = r % WP;
             const bool valid = y < HO && x < HO && a < na;
@@ -376,7 +327,7 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
 #pragma unroll
             for (int b = 0; b < NB; ++b) {
                 float u[16];
-                fm_block_vals<L>(tmem_lane + t * DCOLS + h * (N / 2) + 16 * b, cs + 16 * b, inv, u);
+                fm_block_vals(sacc + l * SROW + h * (N / 2) + 16 * b, cs + 16 * b, inv, u);
                 mx = fmaxf(mx, fm_max16(u));
                 if constexpr (POOL) {
                     fm_xpool(u, odd, cv[t][b]);
@@ -393,7 +344,6 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
             if (valid) atomicMax(&ms->amax[L][a], __float_as_uint(mx));
         }
     }
-    tcgen05_fence_before();
     fm_epi_sync();
     const bool writer = POOL ? (rows_here && !upper) : rows_here;
     if (writer) {
@@ -433,8 +383,8 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
             }
         }
     }
-    fence_proxy_async_smem();
-    fm_arrive_warp(&ms->act_ready);
+    fence_proxy_async_smem();              // st.shared operand rows -> visible to the next layer's wgmma
+    fm_epi_sync();
     FM_ACC(26 + L);
 }
 
@@ -445,28 +395,17 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
     const uint32_t sm_base = smem_u32(sm);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < FM_SLOTS; ++s) { mbar_init(&ms->w_full[s], 1); mbar_init(&ms->w_free[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&ms->acc0_full[b], 1); mbar_init(&ms->acc0_free[b], FM_EPI_WARPS); }
-        mbar_init(&ms->layer_full, 1);
-        mbar_init(&ms->act_ready, FM_EPI_WARPS);
+        for (int s = 0; s < FM_SLOTS; ++s) { mbar_init(&ms->w_full[s], 1); mbar_init(&ms->w_free[s], FM_EPI_WARPS); }
         mbar_init(&ms->xraw_full, 1);
         mbar_init(&ms->xraw_free, FM_EPI_WARPS);
-        ms->xflag[0] = 0; ms->xflag[1] = 0;
         fence_mbar_init();
     }
-    if (warp == 0) tmem_alloc<512>(&ms->tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = ms->tmem_slot;
     const float* __restrict__ cst = A.consts;
-    const bool timing = A.timing != nullptr && blockIdx.x == 0;
-    unsigned long long tacc[40];
-#pragma unroll
-    for (int i = 0; i < 40; ++i) tacc[i] = 0;
+    unsigned long long* tacc = (blockIdx.x == 0 && threadIdx.x == 0) ? A.timing : nullptr;
     griddep_launch_dependents();       // the next kernel of the stream may start its prologue; it still waits for this grid
 
-    if (warp == 1) {
+    if (warp == FM_LOADER_WARP) {
         // ================= loader =================
         if (lane == 0) {
             uint32_t g = 0;
@@ -477,7 +416,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
                     mbar_arrive_expect_tx(&ms->xraw_full, FM_A * 363 * 4);
                     bulk_g2s(sm + FM_XRAW, A.x + (size_t)tile * FM_A * 363, FM_A * 363 * 4, &ms->xraw_full);
                 } else {
-                    fm_arrive(&ms->xraw_full);        // the epilogue warps read this tile straight from global memory
+                    fm_arrive(&ms->xraw_full);        // the compute warps read this tile straight from global memory
                 }
             };
             for (int tile = blockIdx.x; tile < A.num_tiles; tile += gridDim.x, ++it) {
@@ -492,12 +431,12 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
                         if (c == 8) {
                             const int next = tile + gridDim.x;
                             if (next < A.num_tiles) {
-                                fm_wait(&ms->xraw_free, it & 1, 40);
+                                fm_wait(&ms->xraw_free, it & 1);
                                 issue_x(next);
                             }
                         }
                         const uint32_t slot = g % FM_SLOTS, use = g / FM_SLOTS;
-                        if (use >= 1) fm_wait(&ms->w_free[slot], (use - 1) & 1, 20 + slot);
+                        if (use >= 1) fm_wait(&ms->w_free[slot], (use - 1) & 1);
                         const int nu = (units - cc * upc) < upc ? (units - cc * upc) : upc;
                         const uint32_t bytes = (uint32_t)(nu * ub);
                         mbar_arrive_expect_tx(&ms->w_full[slot], bytes);
@@ -507,127 +446,37 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
                 }
             }
         }
-    } else if (warp == 0) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            uint32_t gp = 0, gr = 0;
-            FmIssue is;
-            is.sm16 = sm_base >> 4; is.tmem = tmem; is.slot = 0; is.phase = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < A.num_tiles; tile += gridDim.x, ++it) {
-                // ---- conv0: five pairs of image rows, accumulators double-buffered in TMEM columns [256, 512)
-                {
-                    FM_T0();
-                    fm_wait(&ms->act_ready, gr & 1, 50);
-                    FM_ACC(0);
-                }
-                ++gr;
-                tcgen05_fence_after();
-                const uint32_t has_lo = *reinterpret_cast<volatile uint32_t*>(&ms->xflag[it & 1]);
-                {
-                    {
-                        FM_T0();
-                        fm_wait(&ms->w_full[is.slot], is.phase, 10 + is.slot);
-                        FM_ACC(6);
-                    }
-                    tcgen05_fence_after();
-                    FM_T0();
-                    const uint32_t a_hi = is.sm16 + (FM_R1 >> 4) + fm_lbo_field(2048);
-                    const uint32_t a_lo = a_hi + (fm_lbo(0) >> 4);
-                    const uint32_t bs = is.sm16 + ((FM_RING + is.slot * FM_SLOT_BYTES) >> 4) + fm_lbo_field(512);
-                    for (int j = 0; j < 5; ++j, ++gp) {
-                        const uint32_t b = gp & 1;
-                        if (gp >= 2) {
-                            const long long tw = timing ? clock64() : 0;
-                            fm_wait(&ms->acc0_free[b], ((gp >> 1) - 1) & 1, 52 + b);
-                            if (timing) tacc[32] += (unsigned long long)(clock64() - tw);
-                            tcgen05_fence_after();
-                        }
-                        if (!has_lo) {
-#pragma unroll
-                            for (int tt = 0; tt < 2; ++tt) {
-                                const uint32_t arow = (uint32_t)((2 * j + tt) * 128);       // 16-byte units = rows
-                                const uint32_t d = tmem + 256 + b * 64 + tt * 32;
-#pragma unroll
-                                for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-                                    for (int pr = 0; pr < 2; ++pr)
-                                        fm_mma(d, fm_desc_w(a_hi + arow + (uint32_t)(2 * pr * 128 + kx)),
-                                               fm_desc_w(bs + (((kx * 2 + pr) * 1024) >> 4)), umma_idesc_f16(128, 32), (kx | pr) != 0);
-                            }
-                        } else {
-#pragma unroll
-                            for (int tt = 0; tt < 2; ++tt) {
-                                const uint32_t arow = (uint32_t)((2 * j + tt) * 128);
-                                const uint32_t d = tmem + 256 + b * 64 + tt * 32;
-#pragma unroll
-                                for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-                                    for (int pr = 0; pr < 2; ++pr) {
-                                        const uint32_t aoff = arow + (uint32_t)(2 * pr * 128 + kx);
-                                        const uint64_t db = fm_desc_w(bs + (((kx * 2 + pr) * 1024) >> 4));
-                                        fm_mma(d, fm_desc_w(a_hi + aoff), db, umma_idesc_f16(128, 32), (kx | pr) != 0);
-                                        fm_mma(d, fm_desc_w(a_lo + aoff), db, umma_idesc_f16(128, 32), 1);
-                                    }
-                            }
-                        }
-                        fm_commit(&ms->acc0_full[b]);
-                    }
-                    fm_commit(&ms->w_free[is.slot]);
-                    if (++is.slot == FM_SLOTS) { is.slot = 0; is.phase ^= 1; }
-                    FM_ACC(12);
-                }
-#define FM_ISSUE(Lx)                                   \
-    {                                                  \
-        FM_T0();                                       \
-        fm_wait(&ms->act_ready, gr & 1, 50 + Lx);      \
-        FM_ACC(Lx);                                    \
-    }                                                  \
-    ++gr;                                              \
-    tcgen05_fence_after();                             \
-    fm_issue_layer<Lx>(is, ms, timing, tacc);
-                FM_ISSUE(1) FM_ISSUE(2) FM_ISSUE(3) FM_ISSUE(4) FM_ISSUE(5)
-#undef FM_ISSUE
-                tacc[18] += 1;
-            }
-            if (timing) {
-                for (int i = 0; i < 19; ++i) atomicAdd(&A.timing[i], tacc[i]);
-                atomicAdd(&A.timing[32], tacc[32]);
-            }
-        }
     } else {
-        // ================= epilogue warps =================
-        const int ew = warp - 2, q = warp & 3, h = ew >> 2, et = threadIdx.x - 64;
-        const int l = q * 32 + lane;
-        const uint32_t tmem_lane = tmem + ((uint32_t)(q * 32) << 16);
-        uint32_t gpe = 0, gl = 0;
+        // ================= compute warps: two warpgroups = channel halves h =================
+        const int q = warp & 3, h = warp >> 2, et = threadIdx.x, wt = et & 127;
+        FmRing ring;
+        ring.slot = 0; ring.phase = 0;
         int it = 0;
         if (A.pdl) griddep_wait();         // x (and the feature buffer's previous readers) belong to earlier kernels
         for (int tile = blockIdx.x; tile < A.num_tiles; tile += gridDim.x, ++it) {
             const int na = min(FM_A, A.total_agents - tile * FM_A);
             const bool bulk = A.x_bulk && na == FM_A;
             // ---- inputs: per-agent scale, fp16 split into the padded in0 planes
-            const long long t_conv0 = timing ? clock64() : 0;
+            const long long t_conv0 = tacc ? clock64() : 0;
             if (et < FM_NL * FM_A) (&ms->amax[0][0])[et] = 0;
-            if (et == 64) ms->xflag[(it + 1) & 1] = 0;
+            if (et == 64) ms->xflag = 0;
             fm_zero(sm_base + FM_R2, 2 * fm_planes(1) * fm_lbo(1), et);       // act1 borders
-            if (it == 0) {   // epilogue constants (weights: never produced by the kernel in front of this one); their latency
-                             // hides behind the first input tile's
+            if (it == 0) {   // epilogue constants (weights: never produced by the kernel in front of this one)
                 float* cs = reinterpret_cast<float*>(sm + FM_CST);
                 for (int i = et; i < FM_NL * 2 * 128; i += FM_EPI_THREADS) cs[i] = __ldg(A.consts + i);
             }
-            fm_wait_warp(&ms->xraw_full, it & 1, 41);
+            fm_wait(&ms->xraw_full, it & 1);
             const float* xs = reinterpret_cast<const float*>(sm + FM_XRAW);
             if (!bulk) {
                 // ragged last tile, unaligned or host-mapped inputs: one coalesced pass of plain loads into the same buffer
                 const float* xg = A.x + (size_t)tile * FM_A * 363;
                 float* xw = reinterpret_cast<float*>(sm + FM_XRAW);
-                for (int i = et; i < na * 363; i += FM_EPI_THREADS) xw[i] = __ldg(xg + i);
-                fm_epi_sync();
+                for (int i = et; i < na * 363; i += FM_EPI_THREADS) xw[i] = __ldcg(xg + i);
             }
+            fm_epi_sync();
             {
                 // one warp per agent: scale from max |x|, then the agent's 13 x 16 padded pixels (no barrier in between)
-                const int a = ew;
+                const int a = warp;
                 float m = 0.f;
                 if (a < na)
                     for (int i = lane; i < 363; i += 32) m = fmaxf(m, fabsf(xs[a * 363 + i]));
@@ -663,99 +512,114 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
                     fm_sts16(sm_base + FM_R1 + row * 16, hi);
                     fm_sts16(sm_base + FM_R1 + fm_lbo(0) + row * 16, lo);
                 }
-                if (__any_sync(0xffffffffu, any_lo != 0) && lane == 0) atomicOr(&ms->xflag[it & 1], 1u);
+                if (__any_sync(0xffffffffu, any_lo != 0) && lane == 0) atomicOr(&ms->xflag, 1u);
             }
             fence_proxy_async_smem();
             fm_arrive_warp(&ms->xraw_free);
             fm_epi_sync();                     // xflag / act1 zeroes / in0 complete in every warp
-            fm_arrive_warp(&ms->act_ready);
-            if (timing) tacc[19] += (unsigned long long)(clock64() - t_conv0);
+            if (tacc) atomicAdd(&tacc[19], (unsigned long long)(clock64() - t_conv0));
 
-            // ---- conv0 epilogue: y pairs are the two accumulators of a pair, x pairs neighbouring lanes
+            // ---- conv0: five pairs of image rows (M tiles 2j, 2j + 1 = image rows y = 2j, 2j + 1 of the 8 agents), this
+            //      warpgroup's 16 channels; y pairs are the two accumulators, x pairs rows l ^ 1 = lanes 4 apart
             {
-                const int a = l >> 4, x = l & 15, odd = lane & 1;
-                const float inv = ms->inv0[a], mul = ms->mul1[a];
+                const bool has_lo = ms->xflag != 0;
+                FM_T0();
+                fm_wait(&ms->w_full[ring.slot], ring.phase);
+                FM_ACC(6);
+                const uint32_t a_hi = sm_base + FM_R1, a_lo = a_hi + fm_lbo(0);
+                const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES + h * 16 * 16;
                 const int c0 = h * 16;
-                const float* cs = reinterpret_cast<const float*>(sm + FM_CST) + c0;
-                float k[16], sh[16];
+                const float* cs = reinterpret_cast<const float*>(sm + FM_CST);
+                for (int j = 0; j < 5; ++j) {
+                    float acc[2][2][8];           // [tt][mh]
+                    wgmma_fence();
 #pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const float4 s4 = fm_lds4(cs + i), t4 = fm_lds4(cs + 128 + i);
-                    k[i] = s4.x * inv; k[i + 1] = s4.y * inv; k[i + 2] = s4.z * inv; k[i + 3] = s4.w * inv;
-                    sh[i] = t4.x; sh[i + 1] = t4.y; sh[i + 2] = t4.z; sh[i + 3] = t4.w;
-                }
-                const bool valid = (x & ~1) < 10 && a < na;
-                const int orow0 = fm_aw(1) + a * fm_wp(1) + (x >> 1) + 1;
-                for (int j = 0; j < 5; ++j, ++gpe) {
-                    const uint32_t b = gpe & 1;
-                    {
-                        FM_T0();
-                        fm_wait_warp(&ms->acc0_full[b], (gpe >> 1) & 1, 60 + b);
-                        FM_ACC(20);
-                    }
-                    tcgen05_fence_after();
-                    FM_T0();
-                    const uint32_t col = 256 + b * 64 + c0;
-                    float p0[16], q0[16];
-                    fm_tmem_ld16(tmem_lane + col, p0);
-                    fm_tmem_ld16(tmem_lane + col + 32, q0);
-                    fm_tmem_wait_ld();
-                    tcgen05_fence_before();
-                    fm_arrive_warp(&ms->acc0_free[b]);
-                    if (timing) tacc[33] += (unsigned long long)(clock64() - _t0);
-                    float u[16];
+                    for (int tt = 0; tt < 2; ++tt)
 #pragma unroll
-                    for (int i = 0; i < 16; ++i)
-                        u[i] = fmaxf(fmaxf(fmaf(p0[i], k[i], sh[i]), fmaf(q0[i], k[i], sh[i])), 0.f);
-                    float pp[8];
-                    fm_xpool(u, odd, pp);
-                    if (valid) fm_store8(sm_base + FM_R2, fm_lbo(1), fm_planes(1), orow0 + j * fm_aw(1), (c0 >> 3) + odd, pp, mul);
-                    FM_ACC(26);
+                        for (int mh = 0; mh < 2; ++mh) {
+                            const uint32_t arow = (uint32_t)((2 * j + tt) * 128 + 64 * mh);      // rows of 16 bytes
+#pragma unroll
+                            for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+                                for (int pr = 0; pr < 2; ++pr) {        // K = 16 = image rows ky = 2 pr, 2 pr + 1 (LBO = one row)
+                                    const uint32_t aoff = (arow + 2 * pr * 128 + kx) * 16;
+                                    const uint64_t db = fm_desc(bs + (kx * 2 + pr) * 1024, 512);
+                                    wgmma_f16<16>(acc[tt][mh], fm_desc(a_hi + aoff, 2048), db, (kx | pr) != 0);
+                                    if (has_lo) wgmma_f16<16>(acc[tt][mh], fm_desc(a_lo + aoff, 2048), db, 1);
+                                }
+                        }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+                        for (int i = 0; i < 8; i += 2) {
+                            const int row = 64 * mh + wg_row(wt, i), c = c0 + wg_col(wt, i);
+                            const int a = row >> 4, x = row & 15;
+                            const float inv = ms->inv0[a], mul = ms->mul1[a];
+                            float v[2];
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const float k = cs[c + e] * inv, sh = cs[128 + c + e];
+                                const float u = fmaxf(fmaxf(fmaf(acc[0][mh][i + e], k, sh), fmaf(acc[1][mh][i + e], k, sh)), 0.f);
+                                v[e] = fmaxf(u, __shfl_xor_sync(0xffffffffu, u, 4)) * mul;
+                            }
+                            if ((x & 1) == 0 && x < 10 && a < na) {
+                                const int orow = fm_aw(1) + a * fm_wp(1) + (x >> 1) + 1 + j * fm_aw(1);
+                                const __half2 hh = __floats2half2_rn(v[0], v[1]);
+                                const float2 f = __half22float2(hh);
+                                const __half2 ll = __floats2half2_rn(v[0] - f.x, v[1] - f.y);
+                                const uint32_t addr = sm_base + FM_R2 + (c >> 3) * fm_lbo(1) + orow * 16 + (c & 7) * 2;
+                                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&hh)) : "memory");
+                                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + fm_planes(1) * fm_lbo(1)),
+                                             "r"(*reinterpret_cast<const uint32_t*>(&ll)) : "memory");
+                            }
+                        }
                 }
+                fm_arrive_warp(&ms->w_free[ring.slot]);
+                ring.advance();
                 fence_proxy_async_smem();
-                fm_arrive_warp(&ms->act_ready);
+                fm_epi_sync();
+                FM_ACC(26);
             }
-            fm_epilogue_dyn<1>(sm, sm_base, tmem_lane, ms, na, q, h, lane, et, gl, timing, tacc);
-            fm_epilogue_dyn<2>(sm, sm_base, tmem_lane, ms, na, q, h, lane, et, gl, timing, tacc);
-            fm_epilogue_dyn<3>(sm, sm_base, tmem_lane, ms, na, q, h, lane, et, gl, timing, tacc);
-            fm_epilogue_dyn<4>(sm, sm_base, tmem_lane, ms, na, q, h, lane, et, gl, timing, tacc);
+            fm_epilogue_dyn<1>(sm, sm_base, ms, ring, na, q, h, lane, et, tacc);
+            fm_epilogue_dyn<2>(sm, sm_base, ms, ring, na, q, h, lane, et, tacc);
+            fm_epilogue_dyn<3>(sm, sm_base, ms, ring, na, q, h, lane, et, tacc);
+            fm_epilogue_dyn<4>(sm, sm_base, ms, ring, na, q, h, lane, et, tacc);
             // ---- compress MLP: rows 0..7 of the tile are the agents
             {
+                constexpr int SROW = fm_srow(5);
+                float acc[1][1][32];
+                fm_mma_layer<5>(sm_base, ms, ring, h, acc, tacc);
+                fm_epi_sync();
                 FM_T0();
-                fm_wait_warp(&ms->layer_full, gl & 1, 35);
-                FM_ACC(25);
-            }
-            ++gl;
-            tcgen05_fence_after();
-            const long long t_mlp0 = timing ? clock64() : 0;
-            if (q == 0) {
-                const int a = lane & 7;
-                const float inv = fm_pow2(-fm_scale_exp(ms->amax[4][a]));
-                const float* cs = reinterpret_cast<const float*>(sm + FM_CST) + 5 * 256 + h * 64;
+                float* sacc = reinterpret_cast<float*>(sm + fm_in_base(5));
 #pragma unroll
-                for (int b = 0; b < 4; ++b) {
-                    float u[16];
-                    fm_block_vals<5>(tmem_lane + h * 64 + 16 * b, cs + 16 * b, inv, u);
-                    if (lane < 8 && a < na) {
+                for (int i = 0; i < 32; i += 2) {
+                    const int row = wg_row(wt, i), col = h * 64 + wg_col(wt, i);
+                    if (row < FM_A) *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[0][0][i], acc[0][0][i + 1]);
+                }
+                fm_epi_sync();
+                if (q == 0 && lane < FM_A && lane < na) {
+                    const int a = lane;
+                    const float inv = fm_pow2(-fm_scale_exp(ms->amax[4][a]));
+                    const float* cs = reinterpret_cast<const float*>(sm + FM_CST) + 5 * 256 + h * 64;
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) {
+                        float u[16];
+                        fm_block_vals(sacc + a * SROW + h * 64 + 16 * b, cs + 16 * b, inv, u);
                         float* dst = A.feat + (size_t)(tile * FM_A + a) * 128 + h * 64 + 16 * b;
 #pragma unroll
                         for (int i = 0; i < 16; i += 4)
                             *reinterpret_cast<float4*>(dst + i) = make_float4(u[i], u[i + 1], u[i + 2], u[i + 3]);
                     }
                 }
+                fm_epi_sync();      // every warp is done with this tile's shared state before the next tile resets it
+                FM_ACC(31);
             }
-            tcgen05_fence_before();
-            fm_epi_sync();      // every warp is done with this tile's shared state before the next tile resets it
-            if (timing) tacc[31] += (unsigned long long)(clock64() - t_mlp0);
+            if (tacc) atomicAdd(&tacc[18], 1ull);
         }
-        if (timing && warp == 4 && lane == 0)          // warp 4 = quadrant 0, channel half 0: has work in every layer
-            for (int i = 19; i < 40; ++i)
-                if (i != 32) atomicAdd(&A.timing[i], tacc[i]);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    if (warp == 0) tmem_dealloc<512>(tmem);
 }
 
 // =====================================================================================================================

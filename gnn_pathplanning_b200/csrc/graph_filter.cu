@@ -1,6 +1,6 @@
-// Fused K-tap graph filter for sm_100a (forward + backward).
+// Fused K-tap graph filter for sm_90a (forward + backward).
 //
-// Replaces BatchLSIGF (/root/reference/utils/graphUtils/graphML.py:2273-2367):
+// Replaces BatchLSIGF (gnn_pathplanning/utils/graphUtils/graphML.py:2273-2367):
 //     z_0 = x,  z_k = z_{k-1} . S_b,   y[b,f,n] = sum_{k,g} w[f,0,k,g] z_k[b,g,n] + bias[f]
 // One CTA owns a tile of TS whole samples (R = TS*N node rows):
 //   1. the x rows and the dense GSO tile are staged into shared memory with 1-D bulk
@@ -882,7 +882,7 @@ int launch_gf_forward_tc(const float* x, const void* S, int s_is_f64, const floa
                          float* y, const float* wa, const float* ba, float* logits, int B, int N, int K,
                          int relu, int allow_bulk, cudaStream_t st);
 
-// CTA-pair fp16-split tcgen05 kernel (graph_filter_pair.cu)
+// fp16-split wgmma pair kernel (graph_filter_pair.cu)
 size_t gf_pair_image_bytes(int K);
 bool gf_pair_supported(int N, int K);
 int launch_prep_pair_taps(const float* w, void* img, int K, cudaStream_t st);
@@ -890,8 +890,8 @@ int launch_gf_forward_pair(const float* x, const void* S, int s_is_f64, const vo
                            const float* wa_host, const float* ba_host, float* logits, int B, int N, int K, int relu,
                            cudaStream_t st);
 
-// debug override for the standalone op (gpp_debug_set_option("gf_mode", m)): 0 auto, 1 CUDA-core, 2 tcgen05 3xTF32,
-// 3 tcgen05 CTA-pair fp16-split
+// debug override for the standalone op (gpp_debug_set_option("gf_mode", m)): 0 auto, 1 CUDA-core, 2 wgmma 3xTF32,
+// 3 wgmma pair fp16-split
 static int standalone_gf_mode() { return debug_option(DBG_GF_MODE); }
 }  // namespace gpp
 

@@ -1,71 +1,64 @@
-// CTA-pair tensor-core graph filter for sm_100a: propagate on the CUDA cores, contract on tcgen05 (cta_group::2).
+// Tensor-core graph filter (Hopper wgmma): propagate on the CUDA cores, contract on the tensor cores.
 //
-// Same contract as gf_fwd_kernel / gf_fwd_tc_kernel (BatchLSIGF, /root/reference/utils/graphUtils/graphML.py:2273-2367,
+// Same contract as gf_fwd_kernel / gf_fwd_tc_kernel (BatchLSIGF, reference utils/graphUtils/graphML.py:2273-2367,
 // + the ReLU of decentralplanner.py:221 and optionally the 128->5 action MLP of :303-315), node-major in / out,
 // G = F = 128, K <= 3 taps, small graphs (N nodes known at compile time so the propagation lives in registers).
 //
-// What bounded the round-1 tcgen05 kernel (profiles/r01_ncu_full_summary_tc_filter_b16k.csv) and what changed:
-//   * 393 KB of split taps re-streamed from L2 per 128-row tile by every CTA  ->  the taps are RESIDENT in shared
-//     memory for the whole kernel: two CTAs of a cluster (one TPC) form a pair, each keeps one 64-feature half of the
-//     B operand (96 KB at K = 3) and `tcgen05.mma.cta_group::2` (M = 256: one 128-row tile per CTA) reads both halves.
-//     L2 -> SM traffic per tile drops to the algorithmic bytes (x in, S in, y out).
-//   * 3xTF32 (9.2 K tensor cycles per tile)  ->  2-way fp16 split with power-of-two scaling: v * 2^e = hi + lo, both
-//     fp16 (11 + 11 significant bits, the same 22 bits 3xTF32 keeps), Y += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo at twice
-//     the TF32 rate, half the operand bytes.  fp16 has 5 exponent bits, so the scale is chosen per sample from a bound
-//     on |z_k| (max|x| times powers of the largest absolute column sum of S) by a scout warp that runs one tile ahead
-//     (its read of the x tile is also the L2 prefetch for the producers), per tensor for the taps; both are undone
-//     exactly in the epilogue.  Values more than 2^10 below the per-sample maximum lose relative (not absolute)
-//     precision; nothing can overflow.
-//   * K x 128 accumulator columns + a 12 K-cycle neighbour-sum epilogue that could not overlap the next tile  ->
-//     propagate-then-filter: z_k = z_{k-1}.S is formed BEFORE the GEMM by the producer warps, entirely in registers
-//     (a lane owns 4 features of all N nodes of one sample, so z_2 needs no shared-memory round trip), split and stored
-//     as A-operand rows; ONE 128-column accumulator per tile, double-buffered in TMEM, so the epilogue of tile i
-//     (TMEM -> registers -> scale, bias, ReLU -> swizzled staging -> TMA tensor store / 128->5 logits) overlaps the
-//     MMAs of tile i+1 and the propagation of tile i+2.
+//   * 2-way fp16 split with power-of-two scaling instead of 3xTF32: v * 2^e = hi + lo, both fp16 (11 + 11 significant
+//     bits, the same 22 bits 3xTF32 keeps), Y += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo at twice the TF32 rate, half the
+//     operand bytes.  fp16 has 5 exponent bits, so the scale is chosen per sample from a bound on |z_k| (max|x| times
+//     powers of the largest absolute column sum of S) by scout warps that run one tile ahead, per tensor for the taps;
+//     both are undone exactly in the epilogue.  Values more than 2^10 below the per-sample maximum lose relative (not
+//     absolute) precision; nothing can overflow.
+//   * propagate-then-filter: z_k = x.S^k is formed BEFORE the GEMM by the producer warps, entirely in registers (a
+//     lane owns 4 features of all N nodes of one sample), split and stored as A-operand rows; the dense part is ONE
+//     accumulating GEMM Y[128, 128] = [z_0 | z_1 | z_2][128, 384] . W[384, 128] per tile, and the epilogue is scale,
+//     bias, ReLU and the 5-wide MLP only.
+//   * the taps (fp16 hi | lo, 64 KB per tap) stream through a 2-slot ring of bulk copies, one 32-feature chunk of all
+//     taps per slot; they stay hot in L2.
 //
-// Warp roles (640 threads per CTA): 0-11 producers (x -> z_k -> fp16 hi|lo operand rows), 12-15 epilogue (one TMEM lane
-// quarter each), 16 MMA issuer (one lane; leader CTA only) + TMEM allocation + tap load, 17-19 scouts (S and S.S
-// staging, scales, L2 prefetch).
+// Warp roles (640 threads per CTA): 0-11 producers (x -> z_k -> fp16 hi|lo operand rows), 12-15 = the MMA warpgroup
+// (wgmma into a 128 x 128 register accumulator, then the epilogue straight from its registers), 16 tap loader, 17-19
+// scouts (S and S.S staging, scales, L2 prefetch).
 // Operand row layout: 128 bytes = [32 x hi | 32 x lo] fp16 of one (tap, 32-feature chunk), SWIZZLE_128B K-major; the
 // three products of a K = 16 step differ only in the descriptors' start offsets (+0 / +64 bytes).
 #include "common.cuh"
 #include "tc_common.cuh"
 
-#include <cuda.h>
 #include <cuda_fp16.h>
 
 namespace gpp {
 
 constexpr int GP_THREADS = 640;
 constexpr int GP_PROD_WARPS = 12;           // warps 0..11: 2 ring groups x 3 sample quads x 2 item kinds
-constexpr int GP_EPI_WARP0 = 12;            // warps 12..15: (warp % 4) = TMEM lane quarter
-constexpr int GP_MMA_WARP = 16;
+constexpr int GP_EPI_WARP0 = 12;            // warps 12..15: the MMA + epilogue warpgroup
+constexpr int GP_LOAD_WARP = 16;
 constexpr int GP_SCOUT_WARP0 = 17;          // warps 17..19
 constexpr int GP_SCOUT_WARPS = 3;
 constexpr int GP_M = 128;                   // node rows per CTA tile
 constexpr int GP_C = 128;                   // G = F
 constexpr int GP_NCHUNK = 4;                // 32-feature chunks
-constexpr int GP_BUNIT = (GP_C / 2) * 128;  // one (tap, chunk) B operand half: 64 rows, 8 KB
+constexpr int GP_BUNIT = GP_C * 128;        // one (tap, chunk) B operand: 128 rows, 16 KB
 constexpr int GP_MAX_K = 3;
 constexpr int GP_ACT = 5;
-constexpr int GP_STAGE_BYTES = 2048;        // epilogue staging box: [32 rows][16 cols] fp32
 constexpr int GP_SCALE_RING = 8;            // tiles of per-sample inverse scales kept for the epilogue
 constexpr int GP_MAX_TS = 16;              // samples per tile (128 / N, N >= 8)
-constexpr uint32_t GP_IDESC = umma_idesc_f16(2 * GP_M, GP_C);
+// registers per thread: 96 at launch (640 threads); the three producer warpgroups hand 32 each to the MMA warpgroup,
+// whose 128 x 128 fp32 accumulator alone takes 128
+constexpr int GP_PROD_REGS = 64, GP_MMA_REGS = 192;
+static_assert(3 * GP_PROD_REGS + GP_MMA_REGS + 96 <= 5 * 96, "register pool of the CTA");
 constexpr long long GP_WATCHDOG_CYCLES = 1LL << 31;   // ~1 s: a stuck pipeline traps instead of hanging the GPU
 
 struct GpArgs {
-    CUtensorMap ymap_full;    // y as [rows][128] fp32, box [32 rows][16 cols], SWIZZLE_64B
-    CUtensorMap ymap_tail;    // same, box [(TS*N) % 32 rows][16 cols] (last row block of a full tile)
     const float* x;           // [B*N][128] node-major
     const void* S;            // [B][N][N] f32 / f64
-    const unsigned char* wimg;   // two CTA halves of K*4 operand units (prep_pair_taps_kernel)
+    const unsigned char* wimg;   // K*4 operand units (prep_pair_taps_kernel), unit (k, chunk c) at (c * K + k)
     const float* wscale;      // {2^e, 2^-e} of the taps
     const float* bias;        // [128] or null
     float* y;                 // [B*N][128] or null
     float* logits;            // [N][B][5] or null
-    int B, K, TS, num_tiles, num_pairs;
-    int s_is_f64, relu, has_act, tail_rows;
+    int B, K, TS, num_tiles;
+    int s_is_f64, relu, has_act;
     int ablate;               // debug ("pair_ablate"): 1 skip the propagations, 2 skip the operand stores, 4 skip the x loads, 8 skip the y stores
     unsigned long long* timing;   // optional [16] per-role cycle totals (debug option "tc_timing"), null in production
     float wa[GP_ACT * GP_C];  // action MLP (kernel-parameter constant bank: FFMA operands, no loads)
@@ -81,32 +74,25 @@ __host__ __device__ constexpr int gp_np(int N) { return gp_slot_b(N) + ((N - gp_
 __host__ __device__ constexpr int gp_slot(int N, int n) { return n < gp_na(N) ? n : gp_slot_b(N) + (n - gp_na(N)); }
 
 struct GpSmem {
-    uint32_t b_off, a_off, a_unit, s_off, s_bytes, stage_off, misc_off, bar_off, total;
+    uint32_t b_off, a_off, a_unit, s_off, s_bytes, misc_off, bar_off, total;
     __host__ __device__ GpSmem(int N, int K, int TS) {
-        b_off = 0;
-        a_off = b_off + (uint32_t)K * GP_NCHUNK * GP_BUNIT;
+        b_off = 0;                                          // 2 ring slots of K tap units
+        a_off = b_off + 2u * K * GP_BUNIT;
         // an A operand unit keeps only the 8-row groups that hold tile rows (15 of 16 at N = 10): the MMA still reads
         // 128 rows, i.e. up to 1 KB past the unit -- the next unit or the S buffers, always inside this allocation --
         // and what it computes from them lands in accumulator rows nobody reads
         a_unit = (uint32_t)((TS * N + 7) / 8) * 1024u;
         s_off = a_off + 2u * K * a_unit;
         s_bytes = (uint32_t)TS * N * gp_np(N) * 4 * (K > 2 ? 2 : 1);   // per buffer: S, then S.S (third tap)
-        stage_off = (s_off + 2 * s_bytes + 511u) & ~511u;
-        misc_off = stage_off + 4 * 2 * GP_STAGE_BYTES;     // bias[128] | scale_p[2][TS] | scale_e[8][TS]
+        misc_off = (s_off + 2 * s_bytes + 15u) & ~15u;      // bias[128] | scale_p[2][TS] | scale_e[8][TS]
         bar_off = misc_off + (GP_C + 2 * GP_MAX_TS + GP_SCALE_RING * GP_MAX_TS) * 4;
         total = bar_off + 512;
     }
 };
 
 // ---- mbarrier waits with a watchdog -------------------------------------------------------------------------
-__device__ __noinline__ void gp_watchdog_trap(int id, uint32_t parity) {
-    printf("gf_fwd_pair_kernel: watchdog -- block %d warp %d stuck on barrier %d parity %u\n", (int)blockIdx.x,
-           (int)(threadIdx.x >> 5), id, parity);
-    __trap();
-}
 // try_wait with a suspend-time hint: the waiting thread sleeps in hardware until the phase completes (or the hint
-// elapses) instead of polling -- with plain try_wait loops the seven waiting warps of a CTA executed a third of all
-// issued instructions (profiles/r02_ncu_pair_v2.txt: stall_branch_resolving 2.0, 35.7 K warp instructions per tile).
+// elapses) instead of polling, so waiting warps do not take issue slots from the working ones.
 constexpr uint32_t GP_SUSPEND_HINT_NS = 1000000;
 __device__ __forceinline__ bool gp_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
@@ -119,28 +105,14 @@ __device__ __forceinline__ bool gp_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ bool gp_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity), "r"(GP_SUSPEND_HINT_NS)
-        : "memory");
-    return ok != 0;
-}
+// Watchdog: a barrier that does not complete within ~1 s traps instead of hanging the GPU.  No printf: a function call
+// anywhere in the kernel makes ptxas serialise its wgmma pipelines.  (`id` names the barrier at the call site.)
 __device__ __forceinline__ void gp_wait(uint64_t* bar, uint32_t parity, int id) {
+    (void)id;
     if (gp_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!gp_try_wait(bar, parity))
-        if (clock64() - t0 > GP_WATCHDOG_CYCLES) gp_watchdog_trap(id, parity);
-}
-__device__ __forceinline__ void gp_wait_cluster(uint64_t* bar, uint32_t parity, int id) {
-    if (gp_try_wait_cluster(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!gp_try_wait_cluster(bar, parity))
-        if (clock64() - t0 > GP_WATCHDOG_CYCLES) gp_watchdog_trap(id, parity);
+        if (clock64() - t0 > GP_WATCHDOG_CYCLES) __trap();
 }
 __device__ __forceinline__ void gp_wait_warp(uint64_t* bar, uint32_t parity, int id) {
     if ((threadIdx.x & 31) == 0) gp_wait(bar, parity, id);
@@ -187,7 +159,7 @@ __device__ __forceinline__ void gp_propagate_half(const float* __restrict__ Ms, 
             if (m == 0) {        // first term: no accumulator to clear
                 fmul2_s(sv[i], in[m].x, in[m].y, out[i].x, out[i].y);
                 fmul2_s(sv[i], in[m].z, in[m].w, out[i].z, out[i].w);
-            } else {             // packed FFMA2: half the issue slots of four scalar FMAs, same rounding
+            } else {
                 ffma2_s(sv[i], in[m].x, in[m].y, out[i].x, out[i].y);
                 ffma2_s(sv[i], in[m].z, in[m].w, out[i].z, out[i].w);
             }
@@ -224,8 +196,7 @@ __device__ __forceinline__ void gp_store_rows(const uint32_t (&ahi)[N], uint32_t
 }
 
 template <int N, bool TIMING>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GP_THREADS, 1)
-gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
+__global__ void __launch_bounds__(GP_THREADS, 1) gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
     constexpr int NP = gp_np(N);
     extern __shared__ __align__(1024) unsigned char gp_smem_raw[];
     unsigned char* sm = gp_smem_raw;
@@ -240,122 +211,65 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
     float* scale_p = bias_s + GP_C;                       // [2][GP_MAX_TS]  2^e per sample (producers)
     float* scale_e = scale_p + 2 * GP_MAX_TS;             // [GP_SCALE_RING][GP_MAX_TS]  2^-e (epilogue)
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L.bar_off);
-    // Ring barriers are per group slot.  Only the warps that have an item in a group touch its barriers (3 per CTA at
-    // N = 10), so a warp never waits on groups it has no work in.  a_free has FOUR instances per slot, used round-robin
-    // by (group >> 1) & 3: a warp that only visits every fourth group cannot tell "phase n-1 still running" from
-    // "phase n complete" with a parity wait on a barrier that completes every other group; with an instance that is
-    // reused only every 8 groups the ambiguity cannot arise.
-    uint64_t* a_full = bars;          // [2] leader: the group's item warps (both CTAs) stored all taps of their rows
-    uint64_t* a_free = bars + 2;      // [4][2] the MMAs that read the group have completed (multicast commit)
-    uint64_t* acc_full = bars + 10;   // [2] all MMAs of the tile pair have completed (multicast commit)
-    uint64_t* acc_free = bars + 12;   // [2] leader: 8 epilogue warps (both CTAs) have read the accumulator
+    // Ring barriers are per group slot.  Only the warps that have an item in a group touch its barriers (3 at N = 10),
+    // so a warp never waits on groups it has no work in.  a_free has FOUR instances per slot, used round-robin by
+    // (group >> 1) & 3: a warp that only visits every fourth group cannot tell "phase n-1 still running" from "phase n
+    // complete" with a parity wait on a barrier that completes every other group; with an instance that is reused only
+    // every 8 groups the ambiguity cannot arise.
+    uint64_t* a_full = bars;          // [2] the group's item warps stored all taps of their rows
+    uint64_t* a_free = bars + 2;      // [4][2] the MMAs that read the group have completed
+    uint64_t* b_full = bars + 10;     // [2] the tap units of the group's chunk have landed
+    uint64_t* b_free = bars + 12;     // [2] the MMAs that read them have completed
     uint64_t* s_full = bars + 14;     // [2] the 3 scout warps staged S (+ S.S) + scales of the tile
     uint64_t* s_free = bars + 16;     // [2] 12 producer warps are done with the S buffer
-    uint64_t* b_full = bars + 18;     // this CTA's tap half has landed
-    uint64_t* b_ready = bars + 19;    // leader: both CTAs' tap halves have landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
     const long long t_kernel0 = TIMING ? clock64() : 0;
     unsigned long long tm[4] = {0, 0, 0, 0};          // per-role cycle totals (lane 0 of one warp per role)
 #define GP_T0() const long long _t0 = TIMING ? clock64() : 0
 #define GP_ACC(i) if (TIMING) tm[i] += (unsigned long long)(clock64() - _t0)
+    constexpr int nquad = (TS + 3) >> 2;           // sample quads per tile
+    constexpr int ipg = 2 * nquad;                 // items (producer warps) per group: (quad, kind)
 
     if (tid == 0) {
         for (int i = 0; i < 2; ++i) {
-            mbar_init(&a_full[i], GP_PROD_WARPS);            // the 6 item warps of the group, both CTAs
+            mbar_init(&a_full[i], ipg);
             for (int q4 = 0; q4 < 4; ++q4) mbar_init(&a_free[q4 * 2 + i], 1);
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&acc_free[i], 2 * 4);
+            mbar_init(&b_full[i], 1);
+            mbar_init(&b_free[i], 1);
             mbar_init(&s_full[i], GP_SCOUT_WARPS);
             mbar_init(&s_free[i], GP_PROD_WARPS);
         }
-        mbar_init(b_full, 1);
-        mbar_init(b_ready, 2);
         fence_mbar_init();
     }
-    if (warp == GP_MMA_WARP) {
-        tmem_alloc_cg2<2 * GP_C>(tmem_slot);
-        tmem_relinquish_cg2();
-    }
     for (int i = tid; i < GP_C; i += GP_THREADS) bias_s[i] = a.bias ? a.bias[i] : 0.f;
-    tcgen05_fence_before();
     __syncthreads();
-    cluster_sync_all();           // both CTAs' barriers are initialised before any remote arrive / multicast commit
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp >= GP_MMA_WARP) {
-      if (warp == GP_MMA_WARP) {
-        // =========================== tap load + MMA issuer ===========================
+    if (warp >= GP_LOAD_WARP) {
+      if (warp == GP_LOAD_WARP) {
+        // =========================== tap loader: chunk c of every tap per ring slot ===========================
         if (lane == 0) {
-            const uint32_t bbytes = (uint32_t)K * GP_NCHUNK * GP_BUNIT;
-            mbar_arrive_expect_tx(b_full, bbytes);
-            const unsigned char* src = a.wimg + (size_t)rank * bbytes;
-            for (int u = 0; u < K * GP_NCHUNK; ++u)
-                bulk_g2s(sm + L.b_off + u * GP_BUNIT, src + (size_t)u * GP_BUNIT, GP_BUNIT, b_full);
-            gp_wait(b_full, 0, 12);
-            mbar_arrive_cluster(b_ready, 0);
-            if (rank == 0) {
-                gp_wait_cluster(b_ready, 0, 13);
-                if (TIMING) tm[3] = (unsigned long long)(clock64() - t_kernel0);
-                const long long t_loop0 = TIMING ? clock64() : 0;
-                uint32_t g = 0;
-                int t = 0;
-                for (int p = cluster_id; p < a.num_pairs; p += num_clusters, ++t) {
-                    const int buf = t & 1;
-                    if (t >= 2) {
-                        GP_T0();
-                        gp_wait_cluster(&acc_free[buf], ((t >> 1) - 1) & 1, 6 + buf);
-                        GP_ACC(1);
-                    }
-                    tcgen05_fence_after();
-                    const uint32_t acc = tmem_base + (uint32_t)buf * GP_C;
-                    for (int c = 0; c < GP_NCHUNK; ++c, ++g) {
-                        const int slot = g & 1;
-                        {
-                            GP_T0();
-                            gp_wait_cluster(&a_full[slot], (g >> 1) & 1, slot);
-                            GP_ACC(0);
-                        }
-                        tcgen05_fence_after();
-                        for (int k = 0; k < K; ++k) {
-                            const uint64_t da = umma_desc_sw128(smem_u32(sm + L.a_off + (slot * K + k) * L.a_unit));
-                            const uint64_t db = umma_desc_sw128(smem_u32(sm + L.b_off + (k * GP_NCHUNK + c) * GP_BUNIT));
-                            // descriptor start offsets in 16-byte units: +2 per K = 16 step, +4 = the lo half of the row
-#pragma unroll
-                            for (int ks = 0; ks < 2; ++ks)
-                                umma_f16_cg2(acc, da + 2 * ks, db + 2 * ks, GP_IDESC, (c | k | ks) != 0);
-#pragma unroll
-                            for (int ks = 0; ks < 2; ++ks) umma_f16_cg2(acc, da + 4 + 2 * ks, db + 2 * ks, GP_IDESC, 1u);
-#pragma unroll
-                            for (int ks = 0; ks < 2; ++ks) umma_f16_cg2(acc, da + 2 * ks, db + 4 + 2 * ks, GP_IDESC, 1u);
-                        }
-                        umma_commit_cg2(&a_free[((g >> 1) & 3) * 2 + slot], 3);
-                    }
-                    umma_commit_cg2(&acc_full[buf], 3);
-                }
-                if (TIMING) tm[2] = (unsigned long long)(clock64() - t_loop0);
-                if (TIMING && a.timing) {
-                    atomicAdd(&a.timing[4], tm[0]); atomicAdd(&a.timing[5], tm[1]); atomicAdd(&a.timing[6], tm[2]);
-                    atomicAdd(&a.timing[13], tm[3]); atomicAdd(&a.timing[11], (unsigned long long)t);
+            const uint32_t gbytes = (uint32_t)K * GP_BUNIT;
+            uint32_t g = 0;
+            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+                for (int c = 0; c < GP_NCHUNK; ++c, ++g) {
+                    const int slot = g & 1;
+                    if (g >= 2) gp_wait(&b_free[slot], ((g >> 1) - 1) & 1, 12 + slot);
+                    mbar_arrive_expect_tx(&b_full[slot], gbytes);
+                    bulk_g2s(sm + L.b_off + slot * gbytes, a.wimg + (size_t)c * gbytes, gbytes, &b_full[slot]);
                 }
             }
         }
         __syncwarp();
       } else {
         // =========================== scouts: S staging + per-sample scales, one tile ahead ===========================
-        // Three warps, each owning every third sample of the tile -- one warp doing all 12 samples in turn was the critical
-        // path of the whole kernel (33 K cycles per tile, profiles/r02_pair_phase_v1.txt); their loads hit L2 thanks to
-        // the bulk prefetch issued two tiles earlier.
+        // Three warps, each owning every third sample of the tile; their loads hit L2 thanks to the bulk prefetch
+        // issued two tiles earlier.
         const int sw = warp - GP_SCOUT_WARP0;
         for (int i = sw * 32 + lane; i < 2 * (int)(L.s_bytes / 4); i += GP_SCOUT_WARPS * 32)
             reinterpret_cast<float*>(sm + L.s_off)[i] = 0.f;        // pad slots of the staged rows: never written again
         asm volatile("bar.sync 1, %0;" ::"r"(GP_SCOUT_WARPS * 32) : "memory");
         int t = 0;
-        for (int p = cluster_id; p < a.num_pairs; p += num_clusters, ++t) {
-            const int tile = 2 * p + (int)rank;
+        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++t) {
             const int s0 = tile * TS;
             const int ns = max(0, min(TS, a.B - s0));
             const int sb = t & 1;
@@ -367,8 +281,8 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
             const long long t_work0 = TIMING ? clock64() : 0;
             if (sw == 0 && lane == 0) {
                 // pull the x rows and GSOs of the tile after next into L2: this role's own loads then wait for L2, not for
-                // HBM (the pipeline skeleton alone took 5.6 us per tile waiting for them, profiles/r02_pair_phase_v11.txt)
-                const int tile2 = 2 * (p + 2 * num_clusters) + (int)rank;
+                // HBM
+                const int tile2 = tile + 2 * gridDim.x;
                 const long long first = (long long)tile2 * TS;
                 if (first < a.B) {
                     const long long cnt = min((long long)TS, (long long)a.B - first);
@@ -452,7 +366,7 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
                 }
                 if (K > 2 && v) {
                     // S.S for the third tap: z_2 = (x.S).S = x.(S.S), so the producers form every tap straight from x
-                    // lane = (row m, 4-slot part of the staged row): 1 scalar + 1 vector load and 2 FFMA2 per term
+                    // lane = (row m, 4-slot part of the staged row): 1 scalar + 1 vector load and 4 FMAs per term
                     float* S2d = Sd + TS * N * NP;
                     constexpr int PARTS = NP / 4;
                     static_assert(N * PARTS <= 32, "one lane per (row, 4-slot part)");
@@ -481,108 +395,116 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
         if (TIMING && a.timing && lane == 0 && sw == 0) { atomicAdd(&a.timing[9], tm[0]); atomicAdd(&a.timing[10], tm[1]); }
       }
     } else if (warp >= GP_EPI_WARP0) {
-          // =========================== epilogue: TMEM -> scale, bias, ReLU -> y (TMA store) / logits ===========================
-        const int q = warp - GP_EPI_WARP0;
-        const int r = q * 32 + lane;                       // TMEM lane = node row of the tile
-        unsigned char* stage = sm + L.stage_off + q * 2 * GP_STAGE_BYTES;
+        // =========================== MMA warpgroup: wgmma -> scale, bias, ReLU -> y / logits ===========================
+        // accumulator acc[mh] = rows 64 mh .. 64 mh + 63 of the tile; element i of thread t is (row 64 mh + wg_row(t, i),
+        // column wg_col(t, i)); the 4 lanes of a quad hold the 128 columns of the same two rows
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(GP_MMA_REGS));
+        const int t_wg = tid - 32 * GP_EPI_WARP0;
         const float inv_w = a.wscale[1];
-        const int full_rows = TS * N;
-        uint32_t nstore = 0;
+        uint32_t g = 0;
         int t = 0;
-        for (int p = cluster_id; p < a.num_pairs; p += num_clusters, ++t) {
-            const int tile = 2 * p + (int)rank;
+        float acc[2][64];
+        const long long t_loop0 = TIMING ? clock64() : 0;
+        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x, ++t) {
             const int s0 = tile * TS;
             const int ns = max(0, min(TS, a.B - s0));
             const int R = ns * N;
-            const int buf = t & 1;
-            {
-                GP_T0();
-                gp_wait_warp(&acc_full[buf], (t >> 1) & 1, 4 + buf);
-                GP_ACC(0);
+            for (int c = 0; c < GP_NCHUNK; ++c, ++g) {
+                const int slot = g & 1;
+                {
+                    GP_T0();
+                    gp_wait(&a_full[slot], (g >> 1) & 1, slot);
+                    gp_wait(&b_full[slot], (g >> 1) & 1, 14 + slot);
+                    GP_ACC(0);
+                }
+                wgmma_fence();
+                for (int k = 0; k < K; ++k) {
+                    const uint32_t sa = smem_u32(sm + L.a_off + (slot * K + k) * L.a_unit);
+                    const uint64_t db = gmma_desc_sw128(smem_u32(sm + L.b_off + (slot * K + k) * GP_BUNIT));
+#pragma unroll
+                    for (int mh = 0; mh < 2; ++mh) {
+                        // descriptor start offsets in 16-byte units: +2 per K = 16 step, +4 = the lo half of the row
+                        const uint64_t da = gmma_desc_sw128(sa + mh * 8192);
+#pragma unroll
+                        for (int ks = 0; ks < 2; ++ks) wgmma_f16<128>(acc[mh], da + 2 * ks, db + 2 * ks, (c | k | ks) != 0);
+#pragma unroll
+                        for (int ks = 0; ks < 2; ++ks) wgmma_f16<128>(acc[mh], da + 4 + 2 * ks, db + 2 * ks, 1u);
+#pragma unroll
+                        for (int ks = 0; ks < 2; ++ks) wgmma_f16<128>(acc[mh], da + 2 * ks, db + 4 + 2 * ks, 1u);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                asm volatile("bar.sync 2, 128;" ::: "memory");      // all four warps' MMAs have completed
+                if (t_wg == 0) {
+                    gp_arrive(&a_free[((g >> 1) & 3) * 2 + slot]);
+                    gp_arrive(&b_free[slot]);
+                }
             }
             const long long t_work0 = TIMING ? clock64() : 0;
-            tcgen05_fence_after();
-            const bool valid = r < R;
-            const int bl = valid ? r / N : 0, n = r - bl * N;
-            const float sc = scale_e[(t & (GP_SCALE_RING - 1)) * GP_MAX_TS + bl] * inv_w;
             const size_t row0 = (size_t)s0 * N;
-            // rows of this warp's 32-row block that belong to the tile; the last tile of the batch is clipped by
-            // the tensor map's row extent instead (rows past B*N are never written)
-            const int rows_w = max(0, min(32, full_rows - 32 * q));
-            const bool last_tile = tile == a.num_tiles - 1;
-            const bool do_store = a.y != nullptr && R > 32 * q && !(a.ablate & 8);
-            float acc5[GP_ACT] = {0.f, 0.f, 0.f, 0.f, 0.f};
-            auto store_chunk = [&](const float (&v)[32], int cb) {
+            const bool do_store = a.y != nullptr && !(a.ablate & 8);
+            const float* scl = scale_e + (t & (GP_SCALE_RING - 1)) * GP_MAX_TS;
+            float acc5[2][2][GP_ACT];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    unsigned char* sbuf = stage + (nstore & 1) * GP_STAGE_BYTES;
-                    if (lane == 0) bulk_wait_group_read<1>();      // the store that last read this buffer is done
-                    __syncwarp();
+            for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-                    for (int j = 0; j < 4; ++j)                     // SWIZZLE_64B: 16-byte chunk j of row r at j ^ ((r >> 1) & 3)
-                        *reinterpret_cast<float4*>(sbuf + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)) =
-                            make_float4(v[h * 16 + 4 * j], v[h * 16 + 4 * j + 1], v[h * 16 + 4 * j + 2], v[h * 16 + 4 * j + 3]);
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0 && do_store) {
-                        const void* map = (rows_w == 32 || last_tile) ? &a.ymap_full : &a.ymap_tail;
-                        tma_store_2d(map, sbuf, cb * 32 + h * 16, (int)(row0 + 32 * q));
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int r = 64 * mh + wg_row(t_wg, 2 * hr);
+                    const bool valid = r < R;
+                    const float sc = scl[valid ? r / N : 0] * inv_w;
+                    float p5[GP_ACT] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+                    for (int jj = 0; jj < 16; ++jj) {
+                        const int i = 4 * jj + 2 * hr, col = wg_col(t_wg, i);
+                        float v0 = fmaf(acc[mh][i], sc, bias_s[col]), v1 = fmaf(acc[mh][i + 1], sc, bias_s[col + 1]);
+                        if (a.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                        if (a.has_act) {
+#pragma unroll
+                            for (int o = 0; o < GP_ACT; ++o)
+                                p5[o] = fmaf(v1, a.wa[o * GP_C + col + 1], fmaf(v0, a.wa[o * GP_C + col], p5[o]));
+                        }
+                        if (do_store && valid)
+                            *reinterpret_cast<float2*>(a.y + (row0 + r) * GP_C + col) = make_float2(v0, v1);
                     }
-                    if (lane == 0) bulk_commit_group();
-                    ++nstore;
+#pragma unroll
+                    for (int o = 0; o < GP_ACT; ++o) acc5[mh][hr][o] = p5[o];
                 }
-            };
-            const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * GP_C);
             if (a.has_act) {
-                // planner mode: the 128 -> 5 action MLP needs compile-time tap indices (constant-bank FFMA operands)
 #pragma unroll
-                for (int cb = 0; cb < 4; ++cb) {
-                    float v[32];
-                    tmem_ld_32x32(tacc + cb * 32, v);
+                for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        v[i] = fmaf(v[i], sc, bias_s[cb * 32 + i]);
-                        if (a.relu) v[i] = fmaxf(v[i], 0.f);
+                    for (int hr = 0; hr < 2; ++hr) {
+                        const int r = 64 * mh + wg_row(t_wg, 2 * hr);
+#pragma unroll
+                        for (int o = 0; o < GP_ACT; ++o) {
+                            float v = acc5[mh][hr][o];
+                            v += __shfl_xor_sync(0xffffffffu, v, 1);
+                            v += __shfl_xor_sync(0xffffffffu, v, 2);
+                            acc5[mh][hr][o] = v;
+                        }
+                        if ((lane & 3) == 0 && r < R) {
+                            const int bl = r / N, n = r - bl * N;
+                            float* lp = a.logits + ((size_t)n * a.B + (s0 + bl)) * GP_ACT;
+#pragma unroll
+                            for (int o = 0; o < GP_ACT; ++o) lp[o] = acc5[mh][hr][o] + a.ba[o];
+                        }
                     }
-#pragma unroll
-                    for (int o = 0; o < GP_ACT; ++o)
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) acc5[o] = fmaf(v[i], a.wa[o * GP_C + cb * 32 + i], acc5[o]);
-                    if (a.y != nullptr) store_chunk(v, cb);
-                }
-            } else {
-#pragma unroll 1
-                for (int cb = 0; cb < 4; ++cb) {
-                    float v[32];
-                    tmem_ld_32x32(tacc + cb * 32, v);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        v[i] = fmaf(v[i], sc, bias_s[cb * 32 + i]);
-                        if (a.relu) v[i] = fmaxf(v[i], 0.f);
-                    }
-                    store_chunk(v, cb);
-                }
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(&acc_free[buf], 0);
-            if (a.has_act && valid) {
-                float* lp = a.logits + ((size_t)n * a.B + (s0 + bl)) * GP_ACT;
-#pragma unroll
-                for (int o = 0; o < GP_ACT; ++o) lp[o] = acc5[o] + a.ba[o];
             }
             if (TIMING) tm[1] += (unsigned long long)(clock64() - t_work0);
         }
-        if (lane == 0) bulk_wait_group<0>();
-        if (TIMING && a.timing && lane == 0 && q == 0) { atomicAdd(&a.timing[7], tm[0]); atomicAdd(&a.timing[8], tm[1]); }
+        if (TIMING) tm[2] = (unsigned long long)(clock64() - t_loop0);
+        if (TIMING && a.timing && t_wg == 0) {
+            atomicAdd(&a.timing[4], tm[0]); atomicAdd(&a.timing[6], tm[2]); atomicAdd(&a.timing[8], tm[1]);
+            atomicAdd(&a.timing[11], (unsigned long long)t);
+        }
     } else {
         // =========================== producers: x -> z_k -> fp16 hi|lo operand rows ===========================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(GP_PROD_REGS));
         // An item = 4 samples x one 32-feature chunk of one tile: lane (ql, l8) owns features 4*l8 .. 4*l8+3 of all N
         // nodes of sample ql.  Every tap is formed straight from x (z_1 = x.S, z_2 = x.(S.S)), one half of the output
         // nodes at a time, so the live state is x (N x 4) + half a tap ((N+2)/2 x 4) + N row addresses.
         constexpr int NA = gp_na(N), NB = N - NA, SLOT_B = gp_slot_b(N);
-        constexpr int nquad = (TS + 3) >> 2;           // sample quads per tile
-        constexpr int ipg = 2 * nquad;                 // items per group: (quad, kind)
         constexpr int ipt = ipg * GP_NCHUNK;           // items per tile
         static_assert(2 * ipg == GP_PROD_WARPS, "producer warps = the items of the two ring groups");
         static_assert((TS % 4) == 0, "item = 4 whole samples");
@@ -593,16 +515,14 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
         // its items are I = w, w + 12, ... of the CTA's sequence (tile I / 24, chunk (I % 24) / 6).
         // lanes 0-7 | 8-15 | 16-23 | 24-31 work for samples 0 | 2 | 1 | 3 of the quad: a 64-bit shared store is served one
         // half-warp at a time, and rows 2 samples (20 rows) apart differ in bit 2 of (row & 7), i.e. land in opposite
-        // 64-byte halves of the 128-byte swizzled row -- every operand store is then conflict-free (with samples 0, 1 in
-        // one half-warp half of the row positions collided: 31 % of the kernel's shared-memory wavefronts were conflicts,
-        // profiles/r02_ncu_pair_v13_summary.txt)
+        // 64-byte halves of the 128-byte swizzled row -- every operand store is then conflict-free
         const int ql = ((lane >> 3) & 1) * 2 + (lane >> 4);
         const int l8 = lane & 7;
         const int slot = warp / ipg;
         const int kind = (warp % ipg) / nquad;
         const int sl = ((warp % ipg) % nquad) * 4 + ql;     // sample of the tile this lane works for, in every item
         int ntile_seq = 0;
-        for (int p = cluster_id; p < a.num_pairs; p += num_clusters) ++ntile_seq;
+        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) ++ntile_seq;
         const int total_items = ntile_seq * ipt;
         uint32_t ahi0[N];                              // operand row addresses of tap 0 (same rows, same slot every item)
         gp_row_addrs<N>(smem_u32(sm + L.a_off + (size_t)slot * K * L.a_unit), sl * N, l8, ahi0);
@@ -614,7 +534,7 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
             const int tt = I / ipt, c = (I - tt * ipt) / ipg;
             const uint32_t g = (uint32_t)(tt * GP_NCHUNK + c);
             const int sb = tt & 1;
-            const int smp = (2 * (cluster_id + tt * num_clusters) + (int)rank) * TS + sl;
+            const int smp = (blockIdx.x + tt * (int)gridDim.x) * TS + sl;
             const bool sv = smp < a.B && !(a.ablate & 4);
             float4 xv[N];
             const float* xp = a.x + ((size_t)smp * N) * GP_C + c * 32 + l8 * 4;
@@ -679,7 +599,7 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
             }
             fence_proxy_async_smem();       // st.shared operand rows -> visible to the tensor cores
             __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(&a_full[slot], 0);
+            if (lane == 0) gp_arrive(&a_full[slot]);
             if (TIMING) {
                 tm[2] += (unsigned long long)(clock64() - t_item0);
                 tm[3] += 1;
@@ -698,16 +618,11 @@ gf_fwd_pair_kernel(const __grid_constant__ GpArgs a) {
         atomicAdd(&a.timing[12], (unsigned long long)(clock64() - t_kernel0));
         atomicAdd(&a.timing[14], 1ull);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    cluster_sync_all();           // no CTA leaves (or frees TMEM) while its peer can still arrive on its barriers
-    tcgen05_fence_after();
-    if (warp == GP_MMA_WARP) tmem_dealloc_cg2<2 * GP_C>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------
-// tap images: w [F][1][K][G] -> per CTA half (64 output features) K*4 units of 64 rows x 128 bytes [hi 32 | lo 32]
-// fp16 of w * 2^e, SWIZZLE_128B K-major; e from the largest |w| so that |w| * 2^e < 2^15
+// tap images: w [F][1][K][G] -> K*4 units (chunk-major: the K units of one 32-feature chunk are contiguous) of 128 rows x
+// 128 bytes [hi 32 | lo 32] fp16 of w * 2^e, SWIZZLE_128B K-major; e from the largest |w| so that |w| * 2^e < 2^15
 // ---------------------------------------------------------------------------------------
 // largest |w| over the taps: one value per thread, block maximum, atomicMax on the (non-negative) float bits
 __global__ void __launch_bounds__(1024) gp_tap_absmax_kernel(const float* __restrict__ w, int n, unsigned int* __restrict__ maxbits) {
@@ -749,26 +664,25 @@ __global__ void gp_prep_taps_kernel(const float* __restrict__ w, unsigned char* 
     if (idx >= GP_C * K * GP_C) return;
     const int f = idx / (K * GP_C), kg = idx - f * (K * GP_C), k = kg / GP_C, gch = kg - k * GP_C;
     const int c = gch >> 5, l = gch & 31;
-    const int half = f >> 6, fr = f & 63;
     const float v = w[idx] * sc;
     const __half hi = __float2half_rn(v);
     const __half lo = __float2half_rn(v - __half2float(hi));
-    unsigned char* unit = img + (size_t)half * K * GP_NCHUNK * GP_BUNIT + (size_t)(k * GP_NCHUNK + c) * GP_BUNIT;
-    *reinterpret_cast<__half*>(unit + sw128_offset(fr, l >> 3) + (l & 7) * 2) = hi;
-    *reinterpret_cast<__half*>(unit + sw128_offset(fr, 4 + (l >> 3)) + (l & 7) * 2) = lo;
+    unsigned char* unit = img + (size_t)(c * K + k) * GP_BUNIT;
+    *reinterpret_cast<__half*>(unit + sw128_offset(f, l >> 3) + (l & 7) * 2) = hi;
+    *reinterpret_cast<__half*>(unit + sw128_offset(f, 4 + (l >> 3)) + (l & 7) * 2) = lo;
 }
 
 // ---------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------
-size_t gf_pair_image_bytes(int K) { return (size_t)2 * K * GP_NCHUNK * GP_BUNIT + 64; }   // + {scale, 1/scale}
+size_t gf_pair_image_bytes(int K) { return (size_t)K * GP_NCHUNK * GP_BUNIT + 64; }   // + {scale, 1/scale}
 
 // (the producer schedule assumes at most one item per warp per group: ceil(128 / N / 4) <= 8 producer warps)
 bool gf_pair_supported(int N, int K) { return N == 10 && K >= 1 && K <= GP_MAX_K; }
 
 int launch_prep_pair_taps(const float* w, void* img, int K, cudaStream_t st) {
     unsigned char* base = reinterpret_cast<unsigned char*>(img);
-    float* wscale = reinterpret_cast<float*>(base + (size_t)2 * K * GP_NCHUNK * GP_BUNIT);
+    float* wscale = reinterpret_cast<float*>(base + (size_t)K * GP_NCHUNK * GP_BUNIT);
     const int n = GP_C * K * GP_C;
     GPP_CUDA_OK(cudaMemsetAsync(wscale, 0, 16, st));
     gp_tap_absmax_kernel<<<(n + 1023) / 1024, 1024, 0, st>>>(w, n, reinterpret_cast<unsigned int*>(wscale) + 2);
@@ -779,33 +693,6 @@ int launch_prep_pair_taps(const float* w, void* img, int K, cudaStream_t st) {
 }
 
 static unsigned long long* g_pair_timing = nullptr;   // "tc_timing" debug counters
-
-typedef CUresult (*GpEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static GpEncodeTiled gp_encode_fn() {
-    static GpEncodeTiled fn = nullptr;      // a driver entry point: process-wide, not per device
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<GpEncodeTiled>(p);
-    }
-    return fn;
-}
-static int gp_encode_y(CUtensorMap* map, float* y, size_t rows, int box_rows) {
-    GpEncodeTiled enc = gp_encode_fn();
-    GPP_REQUIRE(enc, GPP_ERR_CUDA, "gf_forward_pair: cuTensorMapEncodeTiled is not available from this driver");
-    const cuuint64_t dims[2] = {(cuuint64_t)GP_C, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)GP_C * 4};
-    const cuuint32_t box[2] = {16, (cuuint32_t)box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, y, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    GPP_REQUIRE(r == CUDA_SUCCESS, GPP_ERR_CUDA, "gf_forward_pair: cuTensorMapEncodeTiled failed (%d)", (int)r);
-    return GPP_OK;
-}
 
 // wa_host / ba_host: HOST copies of the action MLP (they travel as kernel parameters), or null
 int launch_gf_forward_pair(const float* x, const void* S, int s_is_f64, const void* wimg, const float* bias, float* y,
@@ -820,13 +707,11 @@ int launch_gf_forward_pair(const float* x, const void* S, int s_is_f64, const vo
     const int TS = GP_M / N;
     a.x = x; a.S = S;
     a.wimg = reinterpret_cast<const unsigned char*>(wimg);
-    a.wscale = reinterpret_cast<const float*>(a.wimg + (size_t)2 * K * GP_NCHUNK * GP_BUNIT);
+    a.wscale = reinterpret_cast<const float*>(a.wimg + (size_t)K * GP_NCHUNK * GP_BUNIT);
     a.bias = bias; a.y = y; a.logits = logits;
     a.B = B; a.K = K; a.TS = TS;
     a.num_tiles = (B + TS - 1) / TS;
-    a.num_pairs = (a.num_tiles + 1) / 2;
     a.s_is_f64 = s_is_f64; a.relu = relu; a.has_act = wa_host ? 1 : 0;
-    a.tail_rows = (TS * N) % 32;
     a.ablate = debug_option(DBG_PAIR_ABLATE);
     a.timing = nullptr;
     if (debug_option(DBG_TC_TIMING)) {
@@ -840,23 +725,16 @@ int launch_gf_forward_pair(const float* x, const void* S, int s_is_f64, const vo
         for (int i = 0; i < GP_ACT * GP_C; ++i) a.wa[i] = wa_host[i];
         for (int i = 0; i < GP_ACT; ++i) a.ba[i] = ba_host[i];
     }
-    if (y) {
-        int rc = gp_encode_y(&a.ymap_full, y, (size_t)B * N, 32);
-        if (rc) return rc;
-        rc = gp_encode_y(&a.ymap_tail, y, (size_t)B * N, a.tail_rows > 0 ? a.tail_rows : 32);
-        if (rc) return rc;
-    }
     const size_t smem = GpSmem(N, K, TS).total;
     GPP_REQUIRE(smem <= 227 * 1024, GPP_ERR_UNSUPPORTED, "gf_forward_pair: %zu bytes of shared memory do not fit", smem);
     static SmemConfig smem_cfg, smem_cfg_t;
-    const int max_clusters = sm_count() / 2;
-    const int clusters = a.num_pairs < max_clusters ? a.num_pairs : max_clusters;
+    const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
     if (a.timing) {
         GPP_CUDA_OK(ensure_dynamic_smem(gf_fwd_pair_kernel<10, true>, smem_cfg_t, smem));
-        gf_fwd_pair_kernel<10, true><<<2 * clusters, GP_THREADS, smem, st>>>(a);
+        gf_fwd_pair_kernel<10, true><<<grid, GP_THREADS, smem, st>>>(a);
     } else {
         GPP_CUDA_OK(ensure_dynamic_smem(gf_fwd_pair_kernel<10, false>, smem_cfg, smem));
-        gf_fwd_pair_kernel<10, false><<<2 * clusters, GP_THREADS, smem, st>>>(a);
+        gf_fwd_pair_kernel<10, false><<<grid, GP_THREADS, smem, st>>>(a);
     }
     GPP_LAUNCH_CHECK();
     return GPP_OK;
@@ -865,10 +743,9 @@ int launch_gf_forward_pair(const float* x, const void* S, int s_is_f64, const vo
 }  // namespace gpp
 
 // debug: per-role cycle totals of gf_fwd_pair_kernel since the last call (filled only with the "tc_timing" option):
-// [0..3] producer warp 0: wait S, wait ring slot, item work, items; [4..6] MMA thread: wait operands, wait accumulator,
-// loop total; [7..8] epilogue warp 0: wait accumulator, work; [9..10] scout: wait S buffer, work; [11] tile pairs
-// (leader MMA threads); [12] kernel cycles (thread 0 of every CTA); [13] leader start-up until the taps landed;
-// [14] CTAs
+// [0..3] producer warp 0: wait S, wait ring slot, item work, items; [4] MMA warpgroup: wait operands, [6] its loop
+// total, [8] its epilogue work; [9..10] scout: wait S buffer, work; [11] tiles; [12] kernel cycles (thread 0 of every
+// CTA); [14] CTAs
 extern "C" int gpp_debug_pair_timing(unsigned long long* out16) {
     if (!gpp::g_pair_timing) return GPP_ERR_INVALID;
     cudaDeviceSynchronize();

@@ -1,8 +1,8 @@
-// Small-batch fused graph filter + action MLP on tcgen05 (N = 10 agents, K <= 3 taps, planner path): the filter of the
-// benchmark configuration (640 node rows), where the CUDA-core kernel spends 9.3 K cycles per CTA in a 10-row x 384 x 64
-// contraction that is latency- and shared-memory-bound (profiles/r01_phase_timing_c2.txt).
+// Small-batch fused graph filter + action MLP on the Hopper tensor cores (wgmma; N = 10 agents, K <= 3 taps, planner
+// path): the filter of the benchmark configuration (640 node rows), where the CUDA-core kernel's 10-row x 384 x 64
+// contraction is latency- and shared-memory-bound.
 //
-//   y = ReLU(sum_k (x S^k) W_k + b),  logits = y Wa^T + ba          (/root/reference/utils/graphUtils/graphML.py:2342-2366,
+//   y = ReLU(sum_k (x S^k) W_k + b),  logits = y Wa^T + ba          (reference: utils/graphUtils/graphML.py:2342-2366,
 //                                                                    graphs/models/decentralplanner.py:221,301-318)
 //
 // One CTA = 6 samples (60 node rows, one M = 64 accumulator tile) x one 64-column half of the F = 128 outputs; the 2 CTAs
@@ -11,9 +11,9 @@
 // K-major planes, 32 KB per tap) is fetched by bulk copies BEFORE the programmatic-launch wait, i.e. while the feature
 // kernel still runs -- with 22 CTAs at the benchmark size they sit on SMs the feature kernel does not use.  After the
 // wait: thread (sample, feature) reads its 10 node values, forms z_1 = x S and z_2 = z_1 S in registers, scales by the
-// sample's power of two, splits into fp16 hi / lo and stores the K operand planes; one thread issues K * 8 pairs of
-// MMAs (A_hi x [W_hi | W_lo] with N = 128, A_lo x W_hi with N = 64); 8 warps read the accumulator, add the halves, apply
-// bias + ReLU and the 64-column part of the 5-wide action MLP.
+// sample's power of two, splits into fp16 hi / lo and stores the K operand planes; warpgroup 0 issues K * 8 pairs of
+// wgmma (A_hi x [W_hi | W_lo] with N = 128, A_lo x W_hi with N = 64, register accumulators), adds the three products,
+// applies bias + ReLU and the 64-column part of the 5-wide action MLP straight from its registers.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -22,11 +22,11 @@
 
 namespace gpp {
 
-constexpr int GS_N = 10, GS_TS = 6, GS_ROWS = GS_N * GS_TS;       // 60 valid rows of the M = 64 tile
-constexpr int GS_THREADS = 768;                                    // thread = (sample, feature)
+constexpr int GS_N = 10, GS_TS = 6;                                // 60 valid rows of the M = 64 tile
+constexpr int GS_THREADS = 384;                                    // thread = (feature, samples s and s + 3)
+constexpr int GS_SPT = GS_TS / (GS_THREADS / 128);                 // samples per thread
 constexpr int GS_W_PLANE = 128 * 16;                               // one K plane of [W_hi | W_lo]: 128 rows x 16 B
 constexpr int GS_Z_LBO = 64 * 16 + 16;                             // z planes padded by one row: conflict-free 2-byte stores
-constexpr int GS_TMEM_COLS = 128;
 
 struct GsSmem {
     int w_off, zhi_off, zlo_off, s_off, wa_off, bias_off, part_off, misc_off, total;
@@ -38,15 +38,14 @@ struct GsSmem {
         s_off = off; off += GS_TS * GS_N * GS_N * 4;
         wa_off = off; off += 5 * 64 * 4;
         bias_off = off; off += 64 * 4;
-        part_off = off; off += 3 * 64 * 8 * 4;          // two 32-column parts of this CTA + the peer CTA's partial logits
+        part_off = off; off += 2 * 64 * 8 * 4;          // this CTA's partial logits + the peer CTA's
         misc_off = off; off += 128;
         total = off;
     }
 };
 
 struct GsMisc {
-    uint64_t w_full, mma_done;
-    uint32_t tmem_slot, pad;
+    uint64_t w_full;
     uint32_t xmax[GS_TS];
     uint32_t colmax[GS_TS];
     float inv[GS_TS];
@@ -64,32 +63,19 @@ struct GsArgs {
     int B, K, num_tiles, s_is_f64, pdl;
 };
 
-__device__ __forceinline__ uint64_t gs_desc(uint32_t addr, uint32_t lbo) {
-    return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)(128 >> 4) << 32) |
-           ((uint64_t)1 << 46);
-}
-__device__ __forceinline__ void gs_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
+// no-swizzle K-major operand: K planes `lbo` bytes apart, 8-row groups 128 bytes apart
+__device__ __forceinline__ uint64_t gs_desc(uint32_t addr, uint32_t lbo) { return gmma_desc_nosw(addr, lbo, 128); }
 __device__ __forceinline__ int gs_scale_exp(uint32_t bits) {       // m * 2^e in [2^9, 2^10)
     if (bits == 0) return 0;
     int e = 9 - ((int)(bits >> 23) - 127);
     return e < -110 ? -110 : (e > 110 ? 110 : e);
 }
 __device__ __forceinline__ float gs_pow2(int e) { return __int_as_float((e + 127) << 23); }
-__device__ __noinline__ void gs_watchdog(int id) {
-    printf("gf_small_mma_kernel: watchdog -- block %d stuck on barrier %d\n", (int)blockIdx.x, id);
-    __trap();
-}
-__device__ __forceinline__ void gs_wait(uint64_t* bar, uint32_t parity, int id) {
+// watchdog: trap after ~1 s instead of hanging the GPU (no printf: a call would serialise the kernel's wgmma)
+__device__ __forceinline__ void gs_wait(uint64_t* bar, uint32_t parity) {
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity))
-        if (clock64() - t0 > 2000000000LL) gs_watchdog(id);
+        if (clock64() - t0 > 2000000000LL) __trap();
 }
 
 template <int K>
@@ -108,7 +94,6 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) gf_sm
     // ---- prologue: nothing here depends on the kernel in front of this one
     if (tid == 0) {
         mbar_init(&ms->w_full, 1);
-        mbar_init(&ms->mma_done, 1);
         fence_mbar_init();
         mbar_arrive_expect_tx(&ms->w_full, (uint32_t)(K * 16 * GS_W_PLANE));
         const unsigned char* src = a.img + (size_t)half * K * 16 * GS_W_PLANE;
@@ -116,41 +101,42 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) gf_sm
             bulk_g2s(sm + L.w_off + k * 16 * GS_W_PLANE, src + (size_t)k * 16 * GS_W_PLANE, 16 * GS_W_PLANE, &ms->w_full);
     }
     if (tid < GS_TS) { ms->xmax[tid] = 0; ms->colmax[tid] = 0; }
-    if (warp == 0) tmem_alloc<GS_TMEM_COLS>(&ms->tmem_slot);
     for (int i = tid; i < 5 * 64; i += GS_THREADS) was[i] = __ldg(a.wa + (i >> 6) * 128 + half * 64 + (i & 63));
     if (tid < 64) biass[tid] = __ldg(a.bias + half * 64 + tid);
     const float inv_w = __ldg(a.cst);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = ms->tmem_slot;
     griddep_launch_dependents();
     if (a.pdl) griddep_wait();           // x = the feature kernel's output
 
-    // ---- operands: thread (sample s, feature f)
-    const int s = tid >> 7, f = tid & 127;
-    const bool live = s < ns;
-    float xv[GS_N];
-    {
+    // ---- operands: thread (sample s, feature f) for s = tid / 128 + 3 * u
+    const int f = tid & 127;
+    float xvs[GS_SPT][GS_N];
+#pragma unroll
+    for (int u = 0; u < GS_SPT; ++u) {
+        const int s = (tid >> 7) + u * (GS_THREADS / 128);
+        const bool live = s < ns;
+        float* xv = xvs[u];
         float m = 0.f;
         const float* xp = a.x + ((size_t)(b0 + s) * GS_N) * 128 + f;
 #pragma unroll
         for (int n = 0; n < GS_N; ++n) {
-            xv[n] = live ? __ldg(xp + n * 128) : 0.f;
+            xv[n] = live ? __ldcg(xp + n * 128) : 0.f;     // L2: written by the kernel this one may overlap (PDL)
             m = fmaxf(m, fabsf(xv[n]));
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
         if (lane == 0) atomicMax(&ms->xmax[s], __float_as_uint(m));
-        if (tid < GS_TS * GS_N * GS_N) {
-            const int sb = tid / (GS_N * GS_N);
-            float v = 0.f;
-            if (sb < ns) {
-                const size_t idx = (size_t)b0 * GS_N * GS_N + tid;
-                v = a.s_is_f64 ? (float)reinterpret_cast<const double*>(a.S)[idx] : reinterpret_cast<const float*>(a.S)[idx];
-            }
-            Ss[tid] = v;
+    }
+    for (int i = tid; i < GS_TS * GS_N * GS_N; i += GS_THREADS) {
+        const int sb = i / (GS_N * GS_N);
+        float v = 0.f;
+        if (sb < ns) {
+            const size_t idx = (size_t)b0 * GS_N * GS_N + i;
+            v = a.s_is_f64 ? (float)reinterpret_cast<const double*>(a.S)[idx] : reinterpret_cast<const float*>(a.S)[idx];
         }
+        Ss[i] = v;
+    }
+    {
         if (K >= 2 && tid < GS_TS * GS_N) {       // largest absolute column sum of each sample's S (thread = one column)
             const int sb = tid / GS_N, n = tid - sb * GS_N;
             if (sb < ns) {
@@ -165,9 +151,11 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) gf_sm
         }
     }
     __syncthreads();
-    {
-        // z_1 = x S, z_2 = z_1 S for this thread's feature: two output nodes per packed FFMA2 (rows of S are read as
-        // 8-byte pairs, the node value is the broadcast scalar)
+#pragma unroll
+    for (int u = 0; u < GS_SPT; ++u) {
+        const int s = (tid >> 7) + u * (GS_THREADS / 128);
+        const float* xv = xvs[u];
+        // z_1 = x S, z_2 = z_1 S for this thread's feature, two output nodes per step (rows of S are read as 8-byte pairs)
         float z1[GS_N], z2[GS_N];
         const float colmax = __uint_as_float(ms->colmax[s]);
         const float* Sp = Ss + s * GS_N * GS_N;
@@ -218,70 +206,57 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) gf_sm
     }
     fence_proxy_async_smem();
     __syncthreads();
-    // ---- MMAs: K * 8 steps of K = 16, accumulator [64 rows][W_hi cols 0..63 | W_lo cols 64..127]
-    if (tid == 0) {
-        gs_wait(&ms->w_full, 0, 1);
-        tcgen05_fence_after();
-        const uint32_t idesc128 = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
-        const uint32_t idesc64 = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
+    // ---- MMAs (warpgroup 0): K * 8 steps of K = 16, accumulators acc [64 rows][W_hi cols 0..63 | W_lo cols 64..127]
+    //      += A_hi x [W_hi | W_lo] and acc_lo [64 rows][64] += A_lo x W_hi (a separate accumulator: wgmma of different
+    //      shapes on the same registers are not ordered)
+    const int nrows = ns * GS_N;
+    if (warp < 4) {
+        float acc[64], acc_lo[32];
+        gs_wait(&ms->w_full, 0);
+        wgmma_fence();
 #pragma unroll
         for (int j = 0; j < K * 8; ++j) {
             const uint64_t db = gs_desc(sm_base + L.w_off + 2 * j * GS_W_PLANE, GS_W_PLANE);
-            gs_mma(tmem, gs_desc(sm_base + L.zhi_off + 2 * j * GS_Z_LBO, GS_Z_LBO), db, idesc128, j > 0);
-            gs_mma(tmem, gs_desc(sm_base + L.zlo_off + 2 * j * GS_Z_LBO, GS_Z_LBO), db, idesc64, 1);
+            wgmma_f16<128>(acc, gs_desc(sm_base + L.zhi_off + 2 * j * GS_Z_LBO, GS_Z_LBO), db, j > 0);
+            wgmma_f16<64>(acc_lo, gs_desc(sm_base + L.zlo_off + 2 * j * GS_Z_LBO, GS_Z_LBO), db, j > 0);
         }
-        umma_commit(&ms->mma_done);
-    }
-    // ---- epilogue: warps 0-7 = (TMEM lane quadrant q, 32-column part hsel); an M = 64 tile keeps row r in lane
-    //      (r % 16) of quadrant r / 16
-    const int nrows = ns * GS_N;
-    if (warp < 8) {
-        const int q = warp & 3, hsel = warp >> 2;
-        if (lane == 0) gs_wait(&ms->mma_done, 0, 2);
-        __syncwarp();
-        tcgen05_fence_after();
-        const int row = q * 16 + (lane & 15);
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + hsel * 32;
-        const int srow = row / GS_N;
-        const float inv = ms->inv[srow < GS_TS ? srow : 0];
-        float p[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-#define GS_LD16(dst, col)                                                                                              \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                                            \
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"                     \
-                 : "=r"(dst[0]), "=r"(dst[1]), "=r"(dst[2]), "=r"(dst[3]), "=r"(dst[4]), "=r"(dst[5]), "=r"(dst[6]),     \
-                   "=r"(dst[7]), "=r"(dst[8]), "=r"(dst[9]), "=r"(dst[10]), "=r"(dst[11]), "=r"(dst[12]), "=r"(dst[13]), \
-                   "=r"(dst[14]), "=r"(dst[15])                                                                        \
-                 : "r"(taddr + (col))                                                                                  \
-                 : "memory")
+        wgmma_commit();
+        wgmma_wait<0>();
+        // ---- epilogue: element i (< 32) of this thread is (row, col) in acc and acc_lo, with its W_lo partner at acc[i + 32];
+        //      the 4 lanes of a quad hold the 64 columns of the same two rows
+        float p[2][5] = {{0.f, 0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f, 0.f}};
+        const int r0 = wg_row(tid, 0);
+        const float inv0 = ms->inv[min(r0 / GS_N, GS_TS - 1)], inv1 = ms->inv[min((r0 + 8) / GS_N, GS_TS - 1)];
 #pragma unroll
-        for (int h16 = 0; h16 < 2; ++h16) {      // 16 columns at a time: A_hi x W_hi + A_lo x W_hi | A_hi x W_lo
-            uint32_t rh[16], rl[16];
-            GS_LD16(rh, h16 * 16);
-            GS_LD16(rl, 64 + h16 * 16);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        for (int i = 0; i < 32; ++i) {
+            const int col = wg_col(tid, i), hr = (i >> 1) & 1;
+            const float y = fmaxf(fmaf((acc[i] + acc_lo[i]) + acc[i + 32], hr ? inv1 : inv0, biass[col]), 0.f);
 #pragma unroll
-            for (int c = 0; c < 16; ++c) {
-                const int col = hsel * 32 + h16 * 16 + c;
-                const float y = fmaxf(fmaf(__uint_as_float(rh[c]) + __uint_as_float(rl[c]), inv, biass[col]), 0.f);
+            for (int q5 = 0; q5 < 5; ++q5) p[hr][q5] = fmaf(y, was[q5 * 64 + col], p[hr][q5]);
+        }
 #pragma unroll
-                for (int q5 = 0; q5 < 5; ++q5) p[q5] = fmaf(y, was[q5 * 64 + col], p[q5]);
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+            for (int q5 = 0; q5 < 5; ++q5) {
+                p[hr][q5] += __shfl_xor_sync(0xffffffffu, p[hr][q5], 1);
+                p[hr][q5] += __shfl_xor_sync(0xffffffffu, p[hr][q5], 2);
             }
-        }
-#undef GS_LD16
-        if (lane < 16 && row < nrows) {
+        if ((lane & 3) == 0) {
 #pragma unroll
-            for (int q5 = 0; q5 < 5; ++q5) part[(hsel * 64 + row) * 8 + q5] = p[q5];
+            for (int hr = 0; hr < 2; ++hr)
+                if (r0 + 8 * hr < nrows)
+#pragma unroll
+                    for (int q5 = 0; q5 < 5; ++q5) part[(r0 + 8 * hr) * 8 + q5] = p[hr][q5];
         }
-        tcgen05_fence_before();
     }
     __syncthreads();
-    // ---- the two 32-column parts in a fixed order -> this CTA's partial logits; CTA 1 of the pair hands its partial
-    //      logits to CTA 0 through distributed shared memory, CTA 0 adds the halves (half 0 first) and the action bias
-    float* peer = part + 2 * 64 * 8;
+    // ---- CTA 1 of the pair hands its partial logits to CTA 0 through distributed shared memory, CTA 0 adds the halves
+    //      (half 0 first) and the action bias
+    float* peer = part + 64 * 8;
     if (half == 1) {
         for (int i = tid; i < nrows * 5; i += GS_THREADS) {
             const int r = i / 5, q5 = i - r * 5;
-            const float v = part[r * 8 + q5] + part[(64 + r) * 8 + q5];
+            const float v = part[r * 8 + q5];
             asm volatile(
                 "{\n\t.reg .b32 ra;\n\t"
                 "mapa.shared::cluster.u32 ra, %0, 0;\n\t"
@@ -295,13 +270,9 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) gf_sm
             const int r = i / 5, q5 = i - r * 5;
             const int b = b0 + r / GS_N, n = r % GS_N;
             a.logits[((size_t)n * a.B + b) * 5 + q5] =
-                (part[r * 8 + q5] + part[(64 + r) * 8 + q5]) + peer[r * 8 + q5] + __ldg(a.ba + q5);
+                part[r * 8 + q5] + peer[r * 8 + q5] + __ldg(a.ba + q5);
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    if (warp == 0) tmem_dealloc<GS_TMEM_COLS>(tmem);
 }
 
 // ---- weight images --------------------------------------------------------------------------------------------------

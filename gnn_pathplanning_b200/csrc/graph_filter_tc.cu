@@ -1,27 +1,26 @@
-// Tensor-core (tcgen05 / TMEM) fused graph filter for sm_100a.
+// Tensor-core (wgmma, Hopper) fused graph filter.
 //
-// Same contract as gf_fwd_kernel (graph_filter.cu; BatchLSIGF, /root/reference/utils/graphUtils/
-// graphML.py:2273-2367, + ReLU + the 128->5 action MLP), node-major input, G = F = 128.
+// Same contract as gf_fwd_kernel (graph_filter.cu; BatchLSIGF, reference utils/graphUtils/graphML.py:2273-2367,
+// + ReLU + the 128->5 action MLP), node-major input, G = F = 128.
 //
 // Algebra: the graph shift acts on the node index and the taps on the feature index, so they commute:
 //     y = sum_k (S^k)^T-shift( x . W_k^T )        instead of        sum_k ( (S^k)^T-shift x ) . W_k^T
-// "filter, then propagate".  The dense part  U = X[128 rows,128] . [W_0^T | ... | W_{K-1}^T]  is ONE
-// GEMM whose A operand is the raw x tile (no per-tap operand to build) and whose K accumulators
-// (128 TMEM columns each) are the per-tap products; the N-term neighbour sums run afterwards on the
-// outputs, straight out of TMEM/shared memory, on the CUDA cores.
+// "filter, then propagate".  Per tap the dense part U_k = X[128 rows,128] . W_k^T is one GEMM whose A operand is the
+// raw x tile (no per-tap operand to build); the N-term neighbour sums of U_k run afterwards on the CUDA cores.
 //
 //   * fp32 parity through split precision (3xTF32): operands are split into hi = tf32(v), lo = tf32(v-hi);
-//     U += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo, fp32 accumulation in TMEM (dropped lo.lo term: 2^-22).
-//   * B operand (taps): pre-split, pre-swizzled 32 KB chunk images (hi | lo) prepared once per weight
-//     update, so a linear copy lands them in the canonical SWIZZLE_128B K-major layout; a 4-stage ring
-//     of 16-byte cp.async (LDGSTS) copies runs one chunk ahead of the MMAs.
-//   * A operand: each 128 x 32 chunk of x is read once from global memory (coalesced float4), split and
-//     stored swizzled into a 2-stage ring; it feeds K chunk-MMAs (one per tap accumulator).
-//   * warp-specialised: 8 producer warps stage operands and arrive on "full" mbarriers; a 9th warp's
-//     elected lane issues tcgen05.mma and releases ring stages with tcgen05.commit -> "done" mbarriers.
-//   * epilogue: U_1.. are copied TMEM -> shared memory (over the idle rings), then every thread owns one
-//     node row x 64 features: U_0 from TMEM + bias + sum_k sum_m S^k[m,n] U_k[m,:], ReLU, optional y
-//     store, and the in-thread 128->5 action reduction (two half-rows combined through shared memory).
+//     U += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo, fp32 accumulation in registers (dropped lo.lo term: 2^-22).
+//   * B operand (taps): pre-split, pre-swizzled 32 KB chunk images (hi | lo) prepared once per weight update, so a
+//     linear copy lands them in the canonical SWIZZLE_128B K-major layout; a 2-stage ring of 16-byte cp.async copies
+//     runs one chunk ahead of the MMAs.
+//   * A operand: each 128 x 32 chunk of x is read from global memory (coalesced float4), split and stored swizzled
+//     into a 2-stage ring.
+//   * warp-specialised: 8 producer warps stage operands and arrive on "full" mbarriers; one MMA warpgroup (warps
+//     8-11) runs wgmma into a 128 x 128 register accumulator (two M = 64 halves), releases ring stages on "done"
+//     mbarriers and, after the 4 chunks of a tap, hands U_k to the producers through shared memory.
+//   * epilogue: every producer thread owns one node row x 64 features: U_0 + bias + sum_k sum_m S^k[m,n] U_k[m,:]
+//     accumulated tap by tap, ReLU, optional y store, and the in-thread 128->5 action reduction (two half-rows
+//     combined through shared memory).
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -29,18 +28,19 @@
 
 namespace gpp {
 
-constexpr int TC_THREADS = 256;
-constexpr int TC_M = 128;                  // node rows per tile (UMMA M)
-constexpr int TC_C = 128;                  // G = F = 128 (UMMA N per tap)
+constexpr int TC_THREADS = 256;           // producer / epilogue threads (+ the MMA warpgroup)
+constexpr int TC_MMA_THREADS = 128;
+constexpr int TC_M = 128;                  // node rows per tile (two wgmma M = 64 halves)
+constexpr int TC_C = 128;                  // G = F = 128 (wgmma N per tap)
 constexpr int TC_CHUNK_K = 32;             // reduction elements per chunk (128 bytes of tf32)
 constexpr int TC_NCC = TC_C / TC_CHUNK_K;  // 4 A chunks per tile
 constexpr int TC_OP_BYTES = TC_M * 128;    // one operand half (hi or lo) of one chunk: 16 KB
 constexpr int TC_STAGE_BYTES = 2 * TC_OP_BYTES;   // hi | lo
-constexpr int TC_NA = 2, TC_NB = 4;        // ring depths
-constexpr int TC_RING_BYTES = (TC_NA + TC_NB) * TC_STAGE_BYTES;   // 192 KB
-constexpr int TC_MAX_K = 4;                // K accumulators x 128 columns <= 512 TMEM columns
+constexpr int TC_NS = 2;                   // ring depth (A and B stages of one item share a slot)
+constexpr int TC_RING_BYTES = 2 * TC_NS * TC_STAGE_BYTES;   // 128 KB
+constexpr int TC_U_BYTES = TC_M * TC_C * 4;                 // U_k handed to the epilogue: 64 KB
+constexpr int TC_MAX_K = 4;
 constexpr int TC_ACT = 5;
-constexpr uint32_t TC_IDESC = umma_idesc_tf32(TC_M, TC_C);
 
 // ---------------------------------------------------------------------------------------
 // B-operand images: img[c] = { hi[128 x 32] , lo[128 x 32] } in SWIZZLE_128B K-major layout; chunk
@@ -79,8 +79,9 @@ struct GfTcSmem {
         sk_floats = (uint32_t)(((K > 1 ? (K - 1) : 0) * TS * N * N + 3) / 4 * 4);
     }
     __host__ __device__ uint32_t a_stage(int s) const { return (uint32_t)s * TC_STAGE_BYTES; }
-    __host__ __device__ uint32_t b_stage(int s) const { return (uint32_t)(TC_NA + s) * TC_STAGE_BYTES; }
-    __host__ __device__ uint32_t sk_off() const { return TC_RING_BYTES; }
+    __host__ __device__ uint32_t b_stage(int s) const { return (uint32_t)(TC_NS + s) * TC_STAGE_BYTES; }
+    __host__ __device__ uint32_t u_off() const { return TC_RING_BYTES; }
+    __host__ __device__ uint32_t sk_off() const { return u_off() + TC_U_BYTES; }
     __host__ __device__ uint32_t misc_off() const { return sk_off() + sk_floats * 4; }   // bias, wa, ba, plog
     __host__ __device__ uint32_t bar_off() const {
         return misc_off() + (TC_C + TC_ACT * TC_C + 8 + TC_M * TC_ACT) * 4;
@@ -104,90 +105,104 @@ __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
     __syncwarp();
 }
 __device__ __forceinline__ void producers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void mma_group_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
 
-// Warp roles: warps 0-7 (256 threads) = producers (B cp.async, A split/store) and epilogue;
-// warp 8 = MMA issuer (one elected lane).  Producers and the issuer only meet on mbarriers, so operand
-// staging for the next chunks overlaps the tensor-core work of the current one.
-__global__ void __launch_bounds__(TC_THREADS + 32, 1) gf_fwd_tc_kernel(const GfTcArgs a) {
+// 128 x 128 accumulator of the MMA warpgroup (acc[h] = rows 64 h .. 64 h + 63) -> U tile in shared memory
+__device__ __forceinline__ void tc_store_u(float* usm, const float (&acc)[2][64], int t) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; i += 2) {
+            const int row = 64 * h + wg_row(t, i), col = wg_col(t, i);
+            *reinterpret_cast<float2*>(usm + usm_off(row, col >> 2) + (col & 3)) = make_float2(acc[h][i], acc[h][i + 1]);
+        }
+}
+
+// Warp roles: warps 0-7 (256 threads) = producers (B cp.async, A split/store) and epilogue; warps 8-11 = MMA
+// warpgroup.  Item q = (tile, tap k, chunk cc) in that order; its A and B operands share ring slot q % 2.
+__global__ void __launch_bounds__(TC_THREADS + TC_MMA_THREADS, 1) gf_fwd_tc_kernel(const GfTcArgs a) {
     extern __shared__ unsigned char smem_raw_tc[];
     const uint32_t raw = smem_u32(smem_raw_tc);
     unsigned char* sm = smem_raw_tc + (((raw + 1023u) & ~1023u) - raw);      // 1024-byte aligned base
     const GfTcSmem L(a.N, a.K, a.TS);
-    float* usm = reinterpret_cast<float*>(sm);                 // epilogue alias of the rings
+    float* usm = reinterpret_cast<float*>(sm + L.u_off());
     float* sk = reinterpret_cast<float*>(sm + L.sk_off());
     float* bias_s = reinterpret_cast<float*>(sm + L.misc_off());
     float* wa_s = bias_s + TC_C;
     float* ba_s = wa_s + TC_ACT * TC_C;
     float* plog = ba_s + 8;                                    // [128][5] partial logits of the upper half-rows
     uint64_t* bars = reinterpret_cast<uint64_t*>(sm + L.bar_off());
-    uint64_t* doneA = bars;                       // [TC_NA] MMAs that read the A stage have completed
-    uint64_t* doneB = bars + TC_NA;               // [TC_NB] MMAs that read the B stage have completed
-    uint64_t* fullA = bars + TC_NA + TC_NB;       // [TC_NA] all producers stored their part of the A chunk
-    uint64_t* fullB = fullA + TC_NA;              // [TC_NB] all producers' cp.async data of the B chunk landed
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(fullB + TC_NB);
+    uint64_t* full = bars;                        // [TC_NS] every producer warp stored its A part and saw its B copies land
+    uint64_t* done = bars + TC_NS;                // [TC_NS] the MMAs that read the slot have completed
+    uint64_t* u_full = bars + 2 * TC_NS;          // U_k of the current tap is in shared memory
+    uint64_t* u_free = u_full + 1;                // the epilogue is done with it
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int N = a.N, K = a.K;
     const int nitems = TC_NCC * K;
 
     if (tid == 0) {
-        for (int i = 0; i < TC_NA + TC_NB; ++i) mbar_init(&bars[i], 1);
-        for (int i = 0; i < TC_NA + TC_NB; ++i) mbar_init(&fullA[i], TC_THREADS / 32);
+        for (int i = 0; i < TC_NS; ++i) {
+            mbar_init(&full[i], TC_THREADS / 32);
+            mbar_init(&done[i], 1);
+        }
+        mbar_init(u_full, 1);
+        mbar_init(u_free, 1);
         fence_mbar_init();
     }
-    if (warp == 0) tmem_alloc<512>(tmem_slot);
     for (int i = tid; i < TC_C; i += blockDim.x) bias_s[i] = a.bias ? a.bias[i] : 0.f;
     if (a.wa) {
         for (int i = tid; i < TC_ACT * TC_C; i += blockDim.x) wa_s[i] = a.wa[i];
         if (tid < TC_ACT) ba_s[tid] = a.ba[tid];
     }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
 
-    if (warp == TC_THREADS / 32) {
-        // =============================== MMA issuer ===============================
-        if (lane == 0) {
-            uint32_t gq = 0, ga = 0;
-            for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
-                for (int it = 0; it < nitems; ++it, ++gq) {
-                    const int cc = it / K, k = it - cc * K;
-                    const int as = ga & 1, bs = gq % TC_NB;
-                    if (k == 0) mbar_wait(&fullA[as], (ga >> 1) & 1);
-                    mbar_wait(&fullB[bs], (gq / TC_NB) & 1);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(sm + L.a_stage(as)), sb = smem_u32(sm + L.b_stage(bs));
-                    const uint64_t a_hi = umma_desc_sw128(sa), a_lo = umma_desc_sw128(sa + TC_OP_BYTES);
-                    const uint64_t b_hi = umma_desc_sw128(sb), b_lo = umma_desc_sw128(sb + TC_OP_BYTES);
-                    const uint32_t acc = tmem_acc + (uint32_t)k * TC_C;
+    if (warp >= TC_THREADS / 32) {
+        // =============================== MMA warpgroup ===============================
+        const int t = tid - TC_THREADS;
+        float acc[2][64];
+        uint32_t q = 0, nu = 0;
+        for (int tile = blockIdx.x; tile < a.num_tiles; tile += gridDim.x) {
+            for (int it = 0; it < nitems; ++it, ++q) {
+                const int cc = it % TC_NCC;
+                const int s = q % TC_NS;
+                mbar_wait(&full[s], (q / TC_NS) & 1);
+                const uint32_t sa = smem_u32(sm + L.a_stage(s)), sb = smem_u32(sm + L.b_stage(s));
+                const uint64_t b_hi = gmma_desc_sw128(sb), b_lo = gmma_desc_sw128(sb + TC_OP_BYTES);
+                wgmma_fence();
 #pragma unroll
-                    for (int ks = 0; ks < TC_CHUNK_K / 8; ++ks)     // +32 bytes (2 x 16 B units) per K = 8 step
-                        umma_tf32(acc, a_hi + 2 * ks, b_hi + 2 * ks, TC_IDESC, (cc | ks) != 0);
-#pragma unroll
-                    for (int ks = 0; ks < TC_CHUNK_K / 8; ++ks)
-                        umma_tf32(acc, a_lo + 2 * ks, b_hi + 2 * ks, TC_IDESC, 1u);
+                for (int h = 0; h < 2; ++h) {
+                    // rows 64 h ..: 8 groups of 1024 bytes further; +32 bytes (2 x 16 B units) per K = 8 step
+                    const uint64_t a_hi = gmma_desc_sw128(sa + h * 8192), a_lo = gmma_desc_sw128(sa + TC_OP_BYTES + h * 8192);
 #pragma unroll
                     for (int ks = 0; ks < TC_CHUNK_K / 8; ++ks)
-                        umma_tf32(acc, a_hi + 2 * ks, b_lo + 2 * ks, TC_IDESC, 1u);
-                    umma_commit(&doneB[bs]);
-                    if (k == K - 1) {
-                        umma_commit(&doneA[as]);
-                        ++ga;
-                    }
+                        wgmma_tf32<128>(acc[h], a_hi + 2 * ks, b_hi + 2 * ks, (cc | ks) != 0);
+#pragma unroll
+                    for (int ks = 0; ks < TC_CHUNK_K / 8; ++ks) wgmma_tf32<128>(acc[h], a_lo + 2 * ks, b_hi + 2 * ks, 1u);
+#pragma unroll
+                    for (int ks = 0; ks < TC_CHUNK_K / 8; ++ks) wgmma_tf32<128>(acc[h], a_hi + 2 * ks, b_lo + 2 * ks, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                mma_group_sync();
+                if (t == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&done[s])) : "memory");
+                if (cc == TC_NCC - 1) {
+                    if (nu >= 1) mbar_wait(u_free, (nu - 1) & 1);
+                    tc_store_u(usm, acc, t);
+                    mma_group_sync();
+                    if (t == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(u_full)) : "memory");
+                    ++nu;
                 }
             }
         }
-        __syncwarp();
     } else {
         // =============================== producers + epilogue ===============================
-        uint32_t gq = 0;    // B chunks of earlier tiles
-        uint32_t ga = 0;    // A chunks produced so far
+        uint32_t q = 0;     // items staged so far
+        uint32_t nu = 0;    // U tiles consumed
         const int j = tid & 7;      // 16-byte column of this thread inside a 128-byte operand row
 
-        auto issue_b = [&](uint32_t q, int c) {
-            const int bs = q % TC_NB;
-            const uint32_t use = q / TC_NB;
-            if (use >= 1) mbar_wait_warp(&doneB[bs], (use - 1) & 1);
+        auto issue_b = [&](uint32_t qq, int c) {      // B chunk c of the tap images -> slot of item qq
+            const int bs = qq % TC_NS;
+            if (qq >= TC_NS) mbar_wait_warp(&done[bs], ((qq / TC_NS) - 1) & 1);
             const char* src = reinterpret_cast<const char*>(a.wimg) + (size_t)c * TC_STAGE_BYTES;
             const uint32_t dst = smem_u32(sm + L.b_stage(bs));
 #pragma unroll
@@ -205,68 +220,41 @@ __global__ void __launch_bounds__(TC_THREADS + 32, 1) gf_fwd_tc_kernel(const GfT
             const int R = ns * N;
             const size_t row0 = (size_t)s0 * N;
             const long long t0 = clock64();
+            const int r = (warp & 3) * 32 + lane;        // node row of the tile
+            const int h = warp >> 2;                     // which 64-feature half of the row
+            float acc[64];
+            long long t_wait = 0, t_prop = 0;
 
-            // the first two B chunks and the first x chunk of this tile go out before anything else
-            issue_b(gq, 0);
+            issue_b(q, 0);                                // item (k 0, cc 0): B chunk k * 4 + cc
             asm volatile("cp.async.commit_group;" ::: "memory");
-            if (nitems > 1) issue_b(gq + 1, (K > 1) ? TC_NCC : 1);      // item 1 = (cc 0, k 1) or (cc 1, k 0)
-            asm volatile("cp.async.commit_group;" ::: "memory");
-            float4 xn[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int r = (tid >> 3) + 32 * i;
-                xn[i] = (r < R) ? __ldg(reinterpret_cast<const float4*>(a.x + (row0 + r) * TC_C + j * 4))
-                                : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-
-            // ---- 4 A chunks x K taps: stage operands; the issuer warp runs U_k += X[:,chunk] . W_k[:,chunk]^T
-            for (int it = 0; it < nitems; ++it) {
-                const int cc = it / K, k = it - cc * K;
-                if (it + 2 < nitems) {                       // B runs two chunks ahead
-                    const int cc2 = (it + 2) / K, k2 = (it + 2) - cc2 * K;
-                    issue_b(gq + it + 2, k2 * TC_NCC + cc2);
-                }
+            for (int it = 0; it < nitems; ++it, ++q) {
+                const int k = it / TC_NCC, cc = it % TC_NCC;
+                if (it + 1 < nitems) issue_b(q + 1, it + 1);   // B runs one item ahead (image chunk index = item index)
                 asm volatile("cp.async.commit_group;" ::: "memory");   // (possibly empty) keeps the group count uniform
-                if (k == 0) {
-                    const int as = ga & 1;
-                    const uint32_t ause = ga >> 1;
-                    if (ause >= 1) mbar_wait_warp(&doneA[as], (ause - 1) & 1);
-                    float4 xv[4];
+                const int as = q % TC_NS;
+                if (q >= TC_NS) mbar_wait_warp(&done[as], ((q / TC_NS) - 1) & 1);
+                unsigned char* stage = sm + L.a_stage(as);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) xv[i] = xn[i];
-                    if (cc + 1 < TC_NCC) {
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int r = (tid >> 3) + 32 * i;
-                            xn[i] = (r < R) ? __ldg(reinterpret_cast<const float4*>(a.x + (row0 + r) * TC_C +
-                                                                                     (cc + 1) * TC_CHUNK_K + j * 4))
-                                            : make_float4(0.f, 0.f, 0.f, 0.f);
-                        }
-                    }
-                    unsigned char* stage = sm + L.a_stage(as);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const int r = (tid >> 3) + 32 * i;
-                        float4 hi, lo;
-                        split_tf32(xv[i].x, hi.x, lo.x);
-                        split_tf32(xv[i].y, hi.y, lo.y);
-                        split_tf32(xv[i].z, hi.z, lo.z);
-                        split_tf32(xv[i].w, hi.w, lo.w);
-                        const uint32_t off = sw128_offset(r, j);
-                        *reinterpret_cast<float4*>(stage + off) = hi;
-                        *reinterpret_cast<float4*>(stage + TC_OP_BYTES + off) = lo;
-                    }
-                    fence_proxy_async_smem();          // st.shared data -> visible to the tensor core
-                    mbar_arrive(&fullA[as]);
-                    ++ga;
+                for (int i = 0; i < 4; ++i) {
+                    const int rr = (tid >> 3) + 32 * i;
+                    const float4 xv = (rr < R) ? __ldg(reinterpret_cast<const float4*>(a.x + (row0 + rr) * TC_C +
+                                                                                     cc * TC_CHUNK_K + j * 4))
+                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+                    float4 hi, lo;
+                    split_tf32(xv.x, hi.x, lo.x);
+                    split_tf32(xv.y, hi.y, lo.y);
+                    split_tf32(xv.z, hi.z, lo.z);
+                    split_tf32(xv.w, hi.w, lo.w);
+                    const uint32_t off = sw128_offset(rr, j);
+                    *reinterpret_cast<float4*>(stage + off) = hi;
+                    *reinterpret_cast<float4*>(stage + TC_OP_BYTES + off) = lo;
                 }
-                asm volatile("cp.async.wait_group 2;" ::: "memory");   // this item's B chunk (3 groups back) landed
-                fence_proxy_async_smem();
-                mbar_arrive(&fullB[(gq + it) % TC_NB]);
-                if (it == 1) {
-                    // GSO tile and its powers: only the epilogue needs them, so they are built here, in the
-                    // shadow of the first chunk-MMAs, not in front of them
-                if (K > 1) {
+                asm volatile("cp.async.wait_group 1;" ::: "memory");   // this item's B chunk landed
+                fence_proxy_async_smem();          // st.shared / cp.async data -> visible to the tensor core
+                mbar_arrive(&full[as]);
+                if (it == 1 && K > 1) {
+                    // GSO tile and its powers: only the epilogue needs them, so they are built here, in the shadow of
+                    // the first chunk-MMAs, not in front of them
                     const size_t off = (size_t)s0 * N * N;
                     const int cnt = ns * N * N;
                     if (a.s_is_f64) {
@@ -283,77 +271,59 @@ __global__ void __launch_bounds__(TC_THREADS + 32, 1) gf_fwd_tc_kernel(const GfT
                         for (int i = tid; i < cnt; i += TC_THREADS) {
                             const int b = i / (N * N), rem = i - b * N * N;
                             const int rr = rem / N, c = rem - rr * N;
-                            float acc = 0.f;
+                            float sacc = 0.f;
                             for (int m = 0; m < N; ++m)
-                                acc = fmaf(prev[b * N * N + rr * N + m], sk[b * N * N + m * N + c], acc);
-                            cur[i] = acc;
+                                sacc = fmaf(prev[b * N * N + rr * N + m], sk[b * N * N + m * N + c], sacc);
+                            cur[i] = sacc;
                         }
                     }
+                    producers_sync();
                 }
-                }
-            }
-            gq += nitems;
-            const long long t1 = clock64();
-
-            // ---- epilogue ---------------------------------------------------------------------------
-            {
-                const uint32_t last = gq - 1;
-                mbar_wait_warp(&doneB[last % TC_NB], (last / TC_NB) & 1);     // every MMA of this tile has completed
-                tcgen05_fence_after();
-                const long long t2 = clock64();
-                const int r = (warp & 3) * 32 + lane;        // TMEM lane = node row of the tile
-                const int h = warp >> 2;                     // which 64-feature half of the row
-                const uint32_t lane_addr = tmem_acc + ((uint32_t)((warp & 3) * 32) << 16);
-                // U_1 .. U_{K-1}: TMEM -> shared memory (aliases the idle operand rings)
-                for (int k = 1; k < K; ++k) {
-                    float* up = usm + (size_t)(k - 1) * TC_M * TC_C;
-#pragma unroll 1
-                    for (int cb = 0; cb < 2; ++cb) {
-                        float v[32];
-                        tmem_ld_32x32(lane_addr + k * TC_C + h * 64 + cb * 32, v);
+                if (cc == TC_NCC - 1) {
+                    // ---- epilogue part of tap k: acc (+)= U_0 + bias, or sum_m S^k[m, n] U_k[(b, m), :]
+                    const long long w0 = clock64();
+                    mbar_wait_warp(u_full, nu & 1);
+                    ++nu;
+                    const long long w1 = clock64();
+                    if (k == 0) {
 #pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            *reinterpret_cast<float4*>(up + usm_off(r, h * 16 + cb * 8 + i)) =
-                                make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-                    }
-                }
-                float acc[64];
-                {
-                    float v[32];
-                    tmem_ld_32x32(lane_addr + h * 64, v);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) acc[i] = v[i] + bias_s[h * 64 + i];
-                    tmem_ld_32x32(lane_addr + h * 64 + 32, v);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) acc[32 + i] = v[i] + bias_s[h * 64 + 32 + i];
-                }
-                tcgen05_fence_before();
-                producers_sync();
-                const long long t3 = clock64();
-                if (r < R) {
-                    const int b = r / N, n = r - b * N;
-                    for (int k = 1; k < K; ++k) {
+                        for (int i = 0; i < 16; ++i) {
+                            const float4 u = ld_smem4(usm + usm_off(r, h * 16 + i));
+                            acc[4 * i] = u.x + bias_s[h * 64 + 4 * i];
+                            acc[4 * i + 1] = u.y + bias_s[h * 64 + 4 * i + 1];
+                            acc[4 * i + 2] = u.z + bias_s[h * 64 + 4 * i + 2];
+                            acc[4 * i + 3] = u.w + bias_s[h * 64 + 4 * i + 3];
+                        }
+                    } else if (r < R) {
+                        const int b = r / N, n = r - b * N;
                         const float* sp = sk + ((size_t)(k - 1) * a.TS + b) * N * N + n;
-                        const float* up = usm + (size_t)(k - 1) * TC_M * TC_C;
                         for (int m = 0; m < N; ++m) {
-                            const float s = sp[m * N];
+                            const float sv = sp[m * N];
                             const int row = b * N + m;
 #pragma unroll
                             for (int i = 0; i < 16; ++i) {
-                                const float4 u = ld_smem4(up + usm_off(row, h * 16 + i));
-                                acc[4 * i] = fmaf(s, u.x, acc[4 * i]);
-                                acc[4 * i + 1] = fmaf(s, u.y, acc[4 * i + 1]);
-                                acc[4 * i + 2] = fmaf(s, u.z, acc[4 * i + 2]);
-                                acc[4 * i + 3] = fmaf(s, u.w, acc[4 * i + 3]);
+                                const float4 u = ld_smem4(usm + usm_off(row, h * 16 + i));
+                                acc[4 * i] = fmaf(sv, u.x, acc[4 * i]);
+                                acc[4 * i + 1] = fmaf(sv, u.y, acc[4 * i + 1]);
+                                acc[4 * i + 2] = fmaf(sv, u.z, acc[4 * i + 2]);
+                                acc[4 * i + 3] = fmaf(sv, u.w, acc[4 * i + 3]);
                             }
                         }
                     }
-                    if (a.relu) {
-#pragma unroll
-                        for (int i = 0; i < 64; ++i) acc[i] = fmaxf(acc[i], 0.f);
-                    }
+                    producers_sync();          // every thread is done with U_k
+                    if (tid == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(u_free)) : "memory");
+                    t_wait += w1 - w0;
+                    t_prop += clock64() - w1;
                 }
-                const long long t4 = clock64();
+            }
+            const long long t1 = clock64();
+
+            // ---- epilogue: ReLU, y, logits ---------------------------------------------------------------
+            {
+                if (r < R && a.relu) {
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) acc[i] = fmaxf(acc[i], 0.f);
+                }
                 if (r < R) {
                     if (a.y) {
                         float4* yp = reinterpret_cast<float4*>(a.y + (row0 + r) * TC_C + h * 64);
@@ -365,48 +335,44 @@ __global__ void __launch_bounds__(TC_THREADS + 32, 1) gf_fwd_tc_kernel(const GfT
                 if (a.wa) {
                     float s5[TC_ACT];
 #pragma unroll
-                    for (int q = 0; q < TC_ACT; ++q) {
-                        float t = 0.f;
+                    for (int qa = 0; qa < TC_ACT; ++qa) {
+                        float tt = 0.f;
 #pragma unroll
                         for (int i = 0; i < 16; ++i) {
-                            const float4 w4 = ld_smem4(wa_s + q * TC_C + h * 64 + 4 * i);
-                            t = fmaf(acc[4 * i], w4.x, t);
-                            t = fmaf(acc[4 * i + 1], w4.y, t);
-                            t = fmaf(acc[4 * i + 2], w4.z, t);
-                            t = fmaf(acc[4 * i + 3], w4.w, t);
+                            const float4 w4 = ld_smem4(wa_s + qa * TC_C + h * 64 + 4 * i);
+                            tt = fmaf(acc[4 * i], w4.x, tt);
+                            tt = fmaf(acc[4 * i + 1], w4.y, tt);
+                            tt = fmaf(acc[4 * i + 2], w4.z, tt);
+                            tt = fmaf(acc[4 * i + 3], w4.w, tt);
                         }
-                        s5[q] = t;
+                        s5[qa] = tt;
                     }
                     if (h == 1) {
 #pragma unroll
-                        for (int q = 0; q < TC_ACT; ++q) plog[r * TC_ACT + q] = s5[q];
+                        for (int qa = 0; qa < TC_ACT; ++qa) plog[r * TC_ACT + qa] = s5[qa];
                     }
                     producers_sync();
                     if (h == 0 && r < R) {
                         const int b = r / N, n = r - b * N;
                         float* lp = a.logits + ((size_t)n * a.B + (s0 + b)) * TC_ACT;
 #pragma unroll
-                        for (int q = 0; q < TC_ACT; ++q) lp[q] = s5[q] + plog[r * TC_ACT + q] + ba_s[q];
+                        for (int qa = 0; qa < TC_ACT; ++qa) lp[qa] = s5[qa] + plog[r * TC_ACT + qa] + ba_s[qa];
                     }
                 }
-                producers_sync();      // the rings (usm alias), sk and plog are free for the next tile
-                const long long t5 = clock64();
-                tacc[0] += t1 - t0; tacc[1] += t2 - t1; tacc[2] += t3 - t2; tacc[3] += t4 - t3; tacc[4] += t5 - t4;
+                producers_sync();      // sk and plog are free for the next tile
+                const long long t2 = clock64();
+                tacc[0] += (t1 - t0) - t_wait - t_prop; tacc[1] += t_wait; tacc[3] += t_prop; tacc[4] += t2 - t1;
                 tacc[5] += 1;
             }
         }
         if (a.timing && tid == 0)
             for (int i = 0; i < 6; ++i) atomicAdd(&a.timing[i], tacc[i]);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    if (warp == 0) tmem_dealloc<512>(tmem_acc);
 }
 
 // ---------------------------------------------------------------------------------------
-// Self-test of the tcgen05 plumbing: D[128][128] = A[128][32] . B[128][32]^T for tf32-exact inputs
-// (descriptor encoding, SWIZZLE_128B addressing, TMEM lane/column mapping) -- used by tests only.
+// Self-test of the wgmma plumbing: D[128][128] = A[128][32] . B[128][32]^T for tf32-exact inputs
+// (descriptor encoding, SWIZZLE_128B addressing, accumulator fragment mapping) -- used by tests only.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const float* __restrict__ A,
                                                                const float* __restrict__ Bm,
@@ -414,14 +380,7 @@ __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const float* __re
     extern __shared__ unsigned char smem_raw_st[];
     const uint32_t raw = smem_u32(smem_raw_st);
     unsigned char* sm = smem_raw_st + (((raw + 1023u) & ~1023u) - raw);
-    uint64_t* bar = reinterpret_cast<uint64_t*>(sm + 2 * TC_OP_BYTES);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 1);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        fence_mbar_init();
-    }
-    if (warp == 0) tmem_alloc<TC_C>(slot);
+    const int tid = threadIdx.x;
     for (int i = tid; i < TC_M * 8; i += 128) {
         const int r = i >> 3, jj = i & 7;
         *reinterpret_cast<float4*>(sm + sw128_offset(r, jj)) = *reinterpret_cast<const float4*>(A + r * 32 + jj * 4);
@@ -429,29 +388,23 @@ __global__ void __launch_bounds__(128, 1) umma_selftest_kernel(const float* __re
             *reinterpret_cast<const float4*>(Bm + r * 32 + jj * 4);
     }
     fence_proxy_async_smem();
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_acc = *slot;
-    if (tid == 0) {
-        const uint32_t sa = smem_u32(sm);
-        const uint64_t da = umma_desc_sw128(sa), db = umma_desc_sw128(sa + TC_OP_BYTES);
+    float acc[2][64];
+    const uint32_t sa = smem_u32(sm);
+    const uint64_t db = gmma_desc_sw128(sa + TC_OP_BYTES);
+    wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) umma_tf32(tmem_acc, da + 2 * ks, db + 2 * ks, TC_IDESC, ks != 0);
-        umma_commit(bar);
-    }
-    mbar_wait(bar, 0);
-    tcgen05_fence_after();
-    const int r = warp * 32 + lane;
-    for (int cb = 0; cb < 4; ++cb) {
-        float v[32];
-        tmem_ld_32x32(tmem_acc + ((uint32_t)(warp * 32) << 16) + cb * 32, v);
+    for (int h = 0; h < 2; ++h) {
+        const uint64_t da = gmma_desc_sw128(sa + h * 8192);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) D[r * TC_C + cb * 32 + i] = v[i];
+        for (int ks = 0; ks < 4; ++ks) wgmma_tf32<128>(acc[h], da + 2 * ks, db + 2 * ks, ks != 0);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<TC_C>(tmem_acc);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 64; ++i) D[(64 * h + wg_row(tid, i)) * TC_C + wg_col(tid, i)] = acc[h][i];
 }
 
 // ---------------------------------------------------------------------------------------
@@ -499,7 +452,7 @@ int launch_gf_forward_tc(const float* x, const void* S, int s_is_f64, const floa
     static SmemConfig smem_cfg;
     GPP_CUDA_OK(ensure_dynamic_smem(gf_fwd_tc_kernel, smem_cfg, smem));
     const int grid = a.num_tiles < sm_count() ? a.num_tiles : sm_count();
-    gf_fwd_tc_kernel<<<grid, TC_THREADS + 32, smem, st>>>(a);
+    gf_fwd_tc_kernel<<<grid, TC_THREADS + TC_MMA_THREADS, smem, st>>>(a);
     GPP_LAUNCH_CHECK();
     return GPP_OK;
 }
@@ -509,7 +462,7 @@ int launch_gf_forward_tc(const float* x, const void* S, int s_is_f64, const floa
 using namespace gpp;
 
 // debug: per-phase cycle totals of gf_fwd_tc_kernel (only filled when GPP_TC_TIMING is set): item staging
-// loop, wait for the last MMA, TMEM->smem/regs, propagation, stores+logits, tiles
+// loop, wait for U_k, (unused), propagation, stores+logits, tiles
 extern "C" int gpp_debug_tc_timing(unsigned long long* out6) {
     if (!g_tc_timing) return GPP_ERR_INVALID;
     cudaDeviceSynchronize();
@@ -520,7 +473,7 @@ extern "C" int gpp_debug_tc_timing(unsigned long long* out6) {
 
 extern "C" int gpp_debug_umma_selftest(const float* A, const float* B, float* D, void* stream) {
     GPP_REQUIRE(A && B && D, GPP_ERR_INVALID, "umma_selftest: null pointer");
-    const size_t smem = 2 * TC_OP_BYTES + 64 + 1024;
+    const size_t smem = 2 * TC_OP_BYTES + 1024;
     GPP_CUDA_OK(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     umma_selftest_kernel<<<1, 128, smem, reinterpret_cast<cudaStream_t>(stream)>>>(A, B, D);
     GPP_LAUNCH_CHECK();

@@ -1,7 +1,7 @@
-// Whole-planner inference for sm_100a: host side of the C ABI (include/gnnpp_b200.h).
+// Whole-planner inference for sm_90a: host side of the C ABI (include/gnnpp_b200.h).
 //
 // Replaces DecentralPlannerNet.addGSO + forward in eval mode
-// (/root/reference/graphs/models/decentralplanner.py:266-318) with two kernels:
+// (gnn_pathplanning/graphs/models/decentralplanner.py:266-318) with two kernels:
 //   feature_kernel  (feature.cu)       per-agent CNN + compress MLP, agents tiled onto CTAs
 //   gf_fwd_kernel   (graph_filter.cu)  K-tap graph filter + ReLU + action MLP, logits out
 // plus the one-off parameter re-layout (k-major filters, eval BatchNorm folded to scale/shift).
@@ -32,10 +32,10 @@ void set_error(const char* fmt, ...) {
 int sm_count() {
     static int cached[kMaxDevices] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev >= 0 && dev < kMaxDevices && cached[dev] > 0) return cached[dev];
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     if (dev >= 0 && dev < kMaxDevices) cached[dev] = n;
     return n;
 }
@@ -59,7 +59,7 @@ int launch_gf_forward_tc(const float* x, const void* S, int s_is_f64, const floa
                          float* y, const float* wa, const float* ba, float* logits, int B, int N, int K,
                          int relu, int allow_bulk, cudaStream_t st);
 
-// CTA-pair fp16-split tcgen05 path (graph_filter_pair.cu)
+// fp16-split wgmma pair path (graph_filter_pair.cu)
 size_t gf_pair_image_bytes(int K);
 bool gf_pair_supported(int N, int K);
 int launch_prep_pair_taps(const float* w, void* img, int K, cudaStream_t st);
@@ -93,7 +93,7 @@ size_t feature_tc_image_floats(int L);
 int launch_prep_feature_tc(const float* w, float* img, int L, cudaStream_t st);
 int launch_feature_tc_kernel(const FeArgs& fa, const float* const* imgs, cudaStream_t st);
 int debug_feature_tc_timing(unsigned long long* out20);
-// small-batch tcgen05 graph filter + action MLP (graph_filter_small.cu)
+// small-batch wgmma graph filter + action MLP (graph_filter_small.cu)
 size_t gf_small_arena_bytes(int K);
 bool gf_small_supported(int N, int K);
 int launch_prep_gf_small(const float* w, float* arena, int K, cudaStream_t st);
@@ -140,11 +140,11 @@ struct gpp_planner {
     float wa_host[5 * 128 + 8];   // host copy of the action MLP: the CTA-pair filter kernel takes it as kernel parameters
     bool pdl_ok;         // the kernels before the next forward in its stream only wrote what it reads after its
                          // griddepcontrol.wait (false right after the weights were re-staged)
-    int gf_mode;         // 0 auto, 1 CUDA-core kernel, 2 tcgen05 3xTF32 kernel, 3 tcgen05 CTA-pair fp16-split kernel
-    int fe_mode;         // feature extractor: 0 auto, 1 CUDA-core kernel, 2 tcgen05 3xTF32 kernel, 3 tcgen05 fp16-split kernel
+    int gf_mode;         // 0 auto, 1 CUDA-core kernel, 2 wgmma 3xTF32 kernel, 3 wgmma pair fp16-split kernel
+    int fe_mode;         // feature extractor: 0 auto, 1 CUDA-core kernel, 2 wgmma 3xTF32 kernel, 3 wgmma fp16-split kernel
     size_t off_fmma;     // images + constants of the fp16-split kernel
-    size_t off_gfsmall;  // tap images of the small-batch tcgen05 graph filter
-    size_t off_fimg[6];  // tcgen05 filter chunk images of conv0..4 and the compress MLP
+    size_t off_gfsmall;  // tap images of the small-batch wgmma graph filter
+    size_t off_fimg[6];  // wgmma filter chunk images of conv0..4 and the compress MLP
     bool weights_set;
     float* raw;          // device staging for host-provided parameters
     size_t raw_floats;
@@ -226,7 +226,7 @@ extern "C" int gpp_planner_create(gpp_planner** out, int K) {
     p->off_gfb = take(128);
     p->off_wa = take(5 * 128);
     p->off_ba = take(64);
-    p->off_gfimg = take(gf_tc_image_floats(K));      // pre-split, pre-swizzled tcgen05 B-operand chunks
+    p->off_gfimg = take(gf_tc_image_floats(K));      // pre-split, pre-swizzled wgmma B-operand chunks
     p->off_gfpair = take(K <= 3 ? gf_pair_image_bytes(K) / 4 + 16 : 16);
     for (int l = 0; l < 6; ++l) p->off_fimg[l] = take(feature_tc_image_floats(l));
     p->off_fmma = take(feature_mma_arena_floats());
@@ -535,7 +535,7 @@ static int planner_forward_impl(gpp_planner* p, const float* x, const void* S, i
     // programmatic dependent launch: each kernel's prologue (barriers, filter prefetch) overlaps the tail of the
     // kernel before it; not for the first forward after the weights changed (the prologue reads them)
     // ... and not on the multi-lane pipelined host path: a dependent kernel launched early parks its CTAs (and their shared
-    // memory) on the SMs the other lane's kernel should be using (45.0 vs 48.4 us per step, profiles/r02_e2e_lanes.txt)
+    // memory) on the SMs the other lane's kernel should be using
     const int pdl = (!debug_option(DBG_NO_PDL) && p->pdl_ok && !p->profiling && !p->lanes_active) ? 1 : 0;
     fa.pdl = pdl;
     fa.w0t = A + p->off_w[0]; fa.w1t = A + p->off_w[1]; fa.w2t = A + p->off_w[2];
@@ -550,10 +550,12 @@ static int planner_forward_impl(gpp_planner* p, const float* x, const void* S, i
         GPP_CUDA_OK(cudaEventRecord(e0, st));
     }
     int rc;
-    // auto = the im2col-free fp16-split tcgen05 kernel from 448 agents (more than 3 per SM): 41 vs 50 us at 640 agents,
-    // 1.23 vs 2.0 ms at 40,960 (profiles/r02_fe_microbench.txt).  One of its tiles costs ~33 us however few agents it
-    // holds, the CUDA-core kernel ~18 us + 6.5 us per agent of a tile, so small batches (the batch-1 rollout step) stay
-    // on the CUDA cores.  The 3xTF32 implicit-GEMM kernel runs on request only.
+    // auto = the im2col-free fp16-split wgmma kernel from 448 agents; small batches (the batch-1 rollout step) stay on the
+    // CUDA cores.  Measured on an H100 SXM (400 W power limit): one launch of 640 agents takes 46-53 us on the CUDA cores
+    // and 53-58 us in the wgmma kernel, but the wgmma kernel holds one tile of 8 agents per CTA (80 CTAs), leaving SMs
+    // to the other batches in flight: bench.py's pipelined value was 14.1-17.0 M agent-steps/s with it against
+    // 14.3-14.4 M with the CUDA-core kernel (alternating runs); at 4,100 agents the wgmma kernel also wins a single
+    // launch (210 vs 232 us).  The 3xTF32 implicit-GEMM kernel runs on request only.
     if (p->fe_mode == 3 || (p->fe_mode == 0 && rows >= 448)) {
         rc = launch_feature_mma_kernel(fa, A + p->off_fmma, allow_bulk, st);
     } else if (p->fe_mode == 2) {
@@ -640,7 +642,7 @@ static void* mapped_alias_cached(gpp_planner* p, const void* host_ptr) {
 }
 
 // kLanes compute lanes (stream + feature workspace + filter scratch each), tickets rotate over them: the batches are
-// independent, so the feature kernel of ticket t+1 (80 of 148 SMs at the benchmark size) runs next to the kernels of
+// independent, so the feature kernel of ticket t+1 (80 of the SMs at the benchmark size) runs next to the kernels of
 // the tickets before it instead of behind them.  `ready`: the inputs are complete once this event has fired.
 static int enqueue_on_lane(gpp_planner* p, const float* x, const void* S, int s_is_f64, float* logits, int B, int N,
                            cudaEvent_t ready, unsigned long long* ticket) {
@@ -707,8 +709,7 @@ extern "C" int gpp_planner_forward_host_async(gpp_planner* p, const float* x_hos
         GPP_CUDA_OK(cudaStreamWaitEvent(p->copy_stream, p->tickets[(t - kStageSlots) % 16], 0));
     {
         const size_t xb = sizeof(float) * nx;
-        // The copy engine moves the step's inputs (stable 35 us per step at 3-6 batches in flight, profiles/r02_e2e_lanes.txt);
-        // the staging kernel that round 1 used (a few CTAs pulling pinned memory with 16-byte loads) needs 5+ batches in
+        // The copy engine moves the step's inputs; the staging kernel (a few CTAs pulling pinned memory with 16-byte loads) needs 5+ batches in
         // flight to match it and is kept behind the "stage_mode" debug option for the probe.
         if (debug_option(DBG_STAGE_MODE) == 0) {
             GPP_CUDA_OK(cudaMemcpyAsync(p->a_x[slot], x_host, xb, cudaMemcpyHostToDevice, p->copy_stream));

@@ -1,10 +1,16 @@
-// tcgen05 / TMEM helpers (sm_100a inline PTX) shared by the tensor-core kernels.
+// Hopper (sm_90a) tensor-core helpers shared by the tensor-core kernels: wgmma with shared-memory operand descriptors,
+// register accumulators, cluster and bulk-copy plumbing.
 //
-// Operand convention used throughout: K-major tiles in the canonical SWIZZLE_128B shared-memory
-// layout -- rows of 128 bytes (32 tf32 values = one K chunk), 8-row groups of 1024 bytes, and
-// inside each row the 16-byte chunk j is stored at position j ^ (row & 7).  Tile bases are
-// 1024-byte aligned.  One tcgen05.mma.kind::tf32 consumes K = 8 (32 bytes): the descriptor's start
-// address advances by 32 bytes per K step inside the 128-byte swizzle atom.
+// Operand convention used throughout: K-major tiles in one of the two canonical shared-memory layouts that wgmma reads
+// through a matrix descriptor --
+//   * SWIZZLE_128B: rows of 128 bytes (32 tf32 or 64 fp16 values = one K chunk), 8-row groups of 1024 bytes, and inside
+//     each row the 16-byte chunk j is stored at position j ^ (row & 7).  Tile bases are 1024-byte aligned.  One K step
+//     (K = 8 tf32 or K = 16 fp16: 32 bytes) advances the descriptor's start address by 32 bytes inside the atom.
+//   * no swizzle ("interleave"): 8 x 16-byte core matrices; rows 16 bytes apart, 8-row groups SBO bytes apart, the two
+//     8-element K halves of a K = 16 step LBO bytes apart.
+// A warpgroup (4 consecutive warps, the first one a multiple of 4) issues wgmma.mma_async for M = 64 rows; thread t of
+// the warpgroup holds accumulator element i at row 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2) and column
+// 8 * (i / 4) + 2 * (t % 4) + i % 2 (wg_row / wg_col).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,80 +22,83 @@ __host__ __device__ __forceinline__ uint32_t sw128_offset(int row, int j) {
     return (uint32_t)(((row >> 3) << 10) + ((row & 7) << 7) + (((j ^ row) & 7) << 4));
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in bits [0,14),
-// leading byte offset >> 4 in [16,30) (=1, unused for swizzled K-major), stride byte offset >> 4 in
-// [32,46) (1024 B between 8-row groups), version 1 in [46,48), layout type SWIZZLE_128B (=2) in [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+// Shared-memory matrix descriptor (GMMA): start address >> 4 in bits [0,14), leading byte offset >> 4 in [16,30),
+// stride byte offset >> 4 in [32,46), layout type in [62,64) (0 = no swizzle, 1 = SWIZZLE_128B).
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ uint64_t gmma_desc_nosw(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
+           ((uint64_t)((sbo >> 4) & 0x3FFF) << 32);
 }
 
-// Instruction descriptor (cute::UMMA::InstrDescriptor) for kind::tf32, fp32 accumulate, A and B
-// K-major: c_format F32 (1) at [4,6), a/b format TF32 (2) at [7,10)/[10,13), N>>3 at [17,23),
-// M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// Accumulator registers and shared-memory operands written by ordinary instructions must be ordered before the
+// wgmma that reads them (the operand writers add fence.proxy.async before their barrier).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
+// accumulator element i of thread `t` (0..127 inside the warpgroup): row in [0, 64), column in [0, N)
+__device__ __forceinline__ int wg_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int wg_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
 
-// Arrives on the mbarrier once every tcgen05 operation issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(bar))
-                 : "memory");
+// D[64 x N] (+)= A[64 x K] . B[N x K]^T, fp32 accumulators d[N / 2]; accumulate = 0 overwrites d.
+#define GPP_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                  "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wgmma_f16_n16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+                 : GPP_D8(0) : "l"(da), "l"(db), "r"(accumulate) : "memory");
 }
+__device__ __forceinline__ void wgmma_f16_n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+                 : GPP_D8(0), GPP_D8(8) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : GPP_D8(0), GPP_D8(8), GPP_D8(16), GPP_D8(24) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : GPP_D8(0), GPP_D8(8), GPP_D8(16), GPP_D8(24), GPP_D8(32), GPP_D8(40), GPP_D8(48), GPP_D8(56) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+                 : GPP_D8(0), GPP_D8(8) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 : GPP_D8(0), GPP_D8(8), GPP_D8(16), GPP_D8(24) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+                 : GPP_D8(0), GPP_D8(8), GPP_D8(16), GPP_D8(24), GPP_D8(32), GPP_D8(40), GPP_D8(48), GPP_D8(56) : "l"(da), "l"(db), "r"(accumulate) : "memory");
+}
+#undef GPP_D8
 
-__device__ __forceinline__ void tcgen05_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma_f16: N");
+    if constexpr (N == 16) wgmma_f16_n16(d, da, db, accumulate);
+    else if constexpr (N == 32) wgmma_f16_n32(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_f16_n64(d, da, db, accumulate);
+    else wgmma_f16_n128(d, da, db, accumulate);
 }
-__device__ __forceinline__ void tcgen05_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// TMEM allocation: one full warp; the base address is written to *slot (shared memory).
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(slot)), "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base lane + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128, "wgmma_tf32: N");
+    if constexpr (N == 32) wgmma_tf32_n32(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_tf32_n64(d, da, db, accumulate);
+    else wgmma_tf32_n128(d, da, db, accumulate);
 }
 
 // fp32 -> (hi, lo) with hi = tf32(x) (round to nearest), lo = tf32(x - hi): x = hi + lo up to 2^-22 |x|
@@ -102,50 +111,6 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     lo = __uint_as_float(l);
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two CTAs of a cluster on one TPC share one MMA of M = 256; each CTA holds its
-// own 128 accumulator rows in its TMEM and its own A rows + one N-half of B in its shared memory.  Issued by the
-// leader CTA (cluster rank 0) only; completion is multicast to the same mbarrier offset in both CTAs.
-// ---------------------------------------------------------------------------------------------------------
-
-// kind::f16 instruction descriptor, fp16 A/B (format 0), fp32 accumulate, both K-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    const uint32_t z = 0;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(z)
-        : "memory");
-}
-
-// arrives (count 1) on the mbarrier at this shared-memory offset in every CTA of `cta_mask` once all tcgen05
-// operations issued so far by this thread have completed
-__device__ __forceinline__ void umma_commit_cg2(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "h"(cta_mask)
-                 : "memory");
-}
-
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* slot) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(slot)), "n"(COLS)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -153,47 +118,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// arrive (count 1) on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  Default semantics
-// (release at CTA scope), as CUTLASS' ClusterBarrier::arrive(cta_id) uses for the same purpose: an explicit
-// .release.cluster compiles to MEMBAR + ERRBAR in front of every arrive (~700 cycles per producer warp per group,
-// profiles/r02_ncu_pair_v2_source_top.txt).  What the peer's tensor core reads (operand rows in the peer's own shared
-// memory) is ordered by the writers' fence.proxy.async before this arrive.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-        ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(cta)
-        : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-
-// 2-D tiled bulk tensor store shared -> global (SASS UTMASTG); c0 = innermost (column) coordinate
-__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(tmap), "r"((uint32_t)__cvta_generic_to_shared(smem_src)), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() {
-    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void bulk_wait_group() {
-    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 }  // namespace gpp

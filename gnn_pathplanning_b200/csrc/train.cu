@@ -1,7 +1,7 @@
-// Training-mode forward and backward of the whole planner for sm_100a (fp32 CUDA cores).
+// Training-mode forward and backward of the whole planner for sm_90a (fp32 CUDA cores).
 //
-// Replaces, in train mode, DecentralPlannerNet.forward (/root/reference/graphs/models/decentralplanner.py
-// :278-318) and the autograd pass behind `loss.backward()` (/root/reference/agents/decentralplannerlocal.py
+// Replaces, in train mode, DecentralPlannerNet.forward (gnn_pathplanning/graphs/models/decentralplanner.py
+// :278-318) and the autograd pass behind `loss.backward()` (gnn_pathplanning/agents/decentralplannerlocal.py
 // :297-314).  The reference calls ConvLayers once PER AGENT, so its BatchNorm batch statistics are taken over
 // (B,H,W) of one agent's slice and the running statistics are updated N times per forward, in agent order;
 // both are reproduced exactly here with all B*N agents batched (image index = b*N + n).

@@ -1,6 +1,6 @@
-"""Drop-in `GraphFilterBatch` / `BatchLSIGF` backed by the sm_100a fused kernel.
+"""Drop-in `GraphFilterBatch` / `BatchLSIGF` backed by the sm_90a fused kernel.
 
-Mirrors the interface of /root/reference/utils/graphUtils/graphML.py:2273-2488 (same
+Mirrors the interface of gnn_pathplanning/utils/graphUtils/graphML.py:2273-2488 (same
 constructor arguments, parameter names/shapes/initialisation, `addGSO`/`forward`
 signatures, the same `assert`s), but the arithmetic runs in libgnnpp_b200.so:
 forward = one fused kernel (propagation + tap contraction + bias [+ ReLU]),
@@ -23,7 +23,7 @@ NODE_MAJOR = _lib.NODE_MAJOR
 def _require_cuda(t: torch.Tensor, name: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
-            "gnn_pathplanning_b200: %s is on %s; this package only has a CUDA (sm_100a) path "
+            "gnn_pathplanning_b200: %s is on %s; this package only has a CUDA (sm_90a) path "
             "and does not fall back to the CPU" % (name, t.device))
 
 

@@ -1,6 +1,6 @@
 """Drop-in `DecentralPlannerNet` backed by libgnnpp_b200.so.
 
-Same module surface as /root/reference/graphs/models/decentralplanner.py:13-318:
+Same module surface as gnn_pathplanning/graphs/models/decentralplanner.py:13-318:
 `DecentralPlannerNet(config)` reading config.num_agents / config.nGraphFilterTaps,
 identical submodule names (`ConvLayers`, `compressMLP`, `GFL`, `actionsMLP`) and hence
 identical `state_dict` keys/shapes and initial values under the same torch seed,
@@ -42,7 +42,7 @@ _CONV_IDX = (0, 4, 7, 11, 14)
 
 
 def weights_init(m):
-    """Same rule as /root/reference/graphs/weights_initializer.py:11-23 (matched on the
+    """Same rule as gnn_pathplanning/graphs/weights_initializer.py:11-23 (matched on the
     class name): Conv* / Linear -> xavier-normal weight (Linear bias 0); BatchNorm* ->
     weight N(1, 0.02), bias 0."""
     name = m.__class__.__name__
@@ -356,13 +356,13 @@ class DecentralPlannerNet(nn.Module):
         return nat
 
     def set_graph_filter_mode(self, mode: str) -> None:
-        """'auto' (default), 'cuda' (fp32 CUDA-core kernel), 'tc' (tcgen05 3xTF32 kernel) or 'pair' (tcgen05
-        CTA-pair fp16-split kernel)."""
+        """'auto' (default), 'cuda' (fp32 CUDA-core kernel), 'tc' (wgmma 3xTF32 kernel) or 'pair' (wgmma
+        fp16-split pair kernel)."""
         self.__dict__["_gf_mode"] = {"auto": 0, "cuda": 1, "tc": 2, "pair": 3}[mode]
 
     def set_feature_mode(self, mode: str) -> None:
-        """Feature extractor kernel: 'auto' (default = 'mma'), 'mma' (tcgen05, fp16 2-way split, im2col-free), 'cuda'
-        (fp32 CUDA cores) or 'tc' (tcgen05 3xTF32 implicit GEMM)."""
+        """Feature extractor kernel: 'auto' (default: 'mma' from 448 agents, else 'cuda'), 'mma' (wgmma, fp16 2-way split, im2col-free), 'cuda'
+        (fp32 CUDA cores) or 'tc' (wgmma 3xTF32 implicit GEMM)."""
         self.__dict__["_fe_mode"] = {"auto": 0, "cuda": 1, "tc": 2, "mma": 3}[mode]
 
     def _forward_fused(self, x, S):
@@ -449,7 +449,7 @@ class DecentralPlannerNet(nn.Module):
         the library's compute lanes and `(ticket, out)` returns at once.  `join(ticket)` makes the current stream wait for
         that step's logits `out` [N,B,5] (device-side, the host does not block), `wait(ticket)` blocks the host.  x, S and
         out must stay untouched until then.  Same arithmetic as `addGSO(S); forward(x)` in eval mode
-        (/root/reference/graphs/models/decentralplanner.py:266-318)."""
+        (gnn_pathplanning/graphs/models/decentralplanner.py:266-318)."""
         assert not self.training, "infer_async is the eval-mode rollout path"
         _require_cuda(x, "x")
         _require_cuda(S, "S")

@@ -12,7 +12,7 @@ partitioned into contiguous episode shards with a full weight replica per GPU:
     stay shard-local (standard DDP semantics; documented in DESIGN.md).
 
 The reference itself has no distributed code (SURVEY.md 2.1); this is new functionality.
-Works with any torch.distributed backend (nccl on the B200 box, gloo in the CPU tests).
+Works with any torch.distributed backend (nccl on GPUs, gloo in the CPU tests).
 """
 from __future__ import annotations
 

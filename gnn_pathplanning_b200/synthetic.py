@@ -5,11 +5,11 @@ DecentralPlannerNet every step:
 
   * the per-agent field-of-view tensor  x [N,3,11,11] f32 in {0,1}
     (map / goal-or-projected-goal / agents-in-view), same semantics as
-    AgentState.toInputTensor (/root/reference/dataloader/statetransformer.py:82-130,
+    AgentState.toInputTensor (gnn_pathplanning/dataloader/statetransformer.py:82-130,
     projected goal :47-66), and
   * the graph shift operator  S = D^-1/2 A D^-1/2,  A = (pairwise distance < r)
     with zero diagonal and the zero-degree guard
-    (/root/reference/utils/multirobotsim_dcenlocal.py:338-348).
+    (gnn_pathplanning/utils/multirobotsim_dcenlocal.py:338-348).
 
 These are input PRODUCERS (SURVEY.md section 8 rows a11/f1/f2), written from the
 behaviour of the reference, pinned against it by tests/golden (the reference

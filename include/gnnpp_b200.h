@@ -1,5 +1,5 @@
 /*
- * gnnpp_b200.h -- C ABI of libgnnpp_b200.so: the B200 (sm_100a) implementation of the
+ * gnnpp_b200.h -- C ABI of libgnnpp_b200.so: the H100 (sm_90a) implementation of the
  * DecentralPlannerNet forward path of proroklab/gnn_pathplanning.
  *
  * The reference has no FFI of its own: its boundary for this path is the PyTorch
@@ -32,7 +32,7 @@ typedef enum gpp_status {
     GPP_ERR_INVALID = -1,     /* bad argument / shape (the reference raises AssertionError) */
     GPP_ERR_UNSUPPORTED = -2, /* valid in the reference but outside this library's envelope */
     GPP_ERR_CUDA = -3,        /* CUDA runtime error (message has the cudaError string) */
-    GPP_ERR_NODEVICE = -4     /* no sm_100 device visible */
+    GPP_ERR_NODEVICE = -4     /* no sm_90 device visible */
 } gpp_status;
 
 /* Tensor layouts of the node-signal tensors x / y. */
@@ -239,20 +239,20 @@ int gpp_planner_wait(gpp_planner* p, unsigned long long ticket);
  * gpp_planner_join(p, ticket, consumer_stream) -- a device-side wait, the host does not block -- or after
  * gpp_planner_wait(ticket).  x, S and logits must stay untouched until then; tickets share the numbering and the limit of
  * 16 outstanding calls with gpp_planner_forward_host_async.  Replaces a loop of `model.addGSO(S); model(x)` calls
- * (/root/reference/agents/decentralplannerlocal.py:576-588) over independent batches. */
+ * (gnn_pathplanning/agents/decentralplannerlocal.py:576-588) over independent batches. */
 int gpp_planner_forward_async(gpp_planner* p, const float* x, const void* S, int s_is_f64, float* logits, int B, int N,
                               void* stream, unsigned long long* ticket);
 int gpp_planner_join(gpp_planner* p, unsigned long long ticket, void* stream);
 
 /* Which graph-filter kernel the planner uses: 0 = automatic (tensor cores once B*N >= 4096 node
- * rows), 1 = CUDA-core fp32 kernel (gf_fwd_kernel), 2 = tcgen05 3xTF32 kernel (gf_fwd_tc_kernel),
- * 3 = tcgen05 CTA-pair fp16-split kernel (gf_fwd_pair_kernel).  GPP_ERR_UNSUPPORTED at forward
+ * rows), 1 = CUDA-core fp32 kernel (gf_fwd_kernel), 2 = wgmma 3xTF32 kernel (gf_fwd_tc_kernel),
+ * 3 = wgmma pair fp16-split kernel (gf_fwd_pair_kernel).  GPP_ERR_UNSUPPORTED at forward
  * time if N / K are outside the requested kernel's envelope. */
 int gpp_planner_set_graph_filter_mode(gpp_planner* p, int mode);
 
 /* Which feature-extractor (CNN + compress MLP) kernel the planner uses: 0 = automatic (currently always the
  * CUDA-core kernel, the faster one at every measured size), 1 = CUDA-core fp32 kernel (feature_kernel),
- * 2 = tcgen05 3xTF32 implicit-GEMM kernel (feature_tc_kernel). */
+ * 2 = wgmma 3xTF32 implicit-GEMM kernel (feature_tc_kernel). */
 int gpp_planner_set_feature_mode(gpp_planner* p, int mode);
 
 /* Per-kernel device timing for the roofline report: when enabled, gpp_planner_forward records

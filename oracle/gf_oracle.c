@@ -1,7 +1,7 @@
 /* CPU ORACLE (plain C) -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * Restates the reference's per-sample-GSO graph filter, BatchLSIGF
- * (/root/reference/utils/graphUtils/graphML.py:2273-2367), element by element:
+ * (gnn_pathplanning/utils/graphUtils/graphML.py:2273-2367), element by element:
  *     z_0 = x ;  z_k[g,n] = sum_m z_{k-1}[g,m] * (float)S[m,n]        (:2350, right-multiply)
  *     y[f,n] = sum_{k,g} h[f,0,k,g] * z_k[g,n] + b[f]                  (:2361-2366)
  * Two variants: f32 storage of every z_k like the reference's float32 tensors with f64

@@ -3,11 +3,11 @@
 A CPU restatement (PyTorch-CPU / numpy) of the one hot path of
 proroklab/gnn_pathplanning that this repo accelerates:
 
-    DecentralPlannerNet.forward      /root/reference/graphs/models/decentralplanner.py:278-318
-    GraphFilterBatch.forward         /root/reference/utils/graphUtils/graphML.py:2458-2477
-    BatchLSIGF                       /root/reference/utils/graphUtils/graphML.py:2273-2367
-    weights_init                     /root/reference/graphs/weights_initializer.py:11-23
-    training loss                    /root/reference/agents/decentralplannerlocal.py:297-312
+    DecentralPlannerNet.forward      gnn_pathplanning/graphs/models/decentralplanner.py:278-318
+    GraphFilterBatch.forward         gnn_pathplanning/utils/graphUtils/graphML.py:2458-2477
+    BatchLSIGF                       gnn_pathplanning/utils/graphUtils/graphML.py:2273-2367
+    weights_init                     gnn_pathplanning/graphs/weights_initializer.py:11-23
+    training loss                    gnn_pathplanning/agents/decentralplannerlocal.py:297-312
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
 legs may import this module.  The product package (gnn_pathplanning_b200) never
@@ -15,11 +15,11 @@ does: it fails loudly when its CUDA library is missing.
 
 PARITY PINNING: the reference ships no tests, golden vectors or fixtures for this
 path (SURVEY.md section 4 / 8c).  The oracle is therefore pinned against outputs of
-the reference itself, imported unmodified in the build container
+the reference itself, imported unmodified by the golden-data generators
 (oracle/ref_shim.py) by tests/golden/make_golden.py; the resulting vectors are
 committed under tests/golden/ and checked by tests/test_oracle_golden.py (CPU) on
-every run, and tests/test_oracle_vs_reference.py re-checks against the live
-reference whenever /root/reference is present.
+every run, and tests/test_oracle_vs_reference.py checks it against further stored
+outputs of the reference (tests/golden/reference_cases.npz).
 
 The op ORDER deliberately follows the reference (N sequential per-agent CNN calls,
 one batched matmul per tap, cat, permute+reshape, one matmul against the flattened

@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- run the reference's own AGENT code (agents/decentralplannerlocal.py,
-utils/multirobotsim_dcenlocal.py, utils/metrics.py, graphs/losses/*) from /root/reference, unmodified,
+utils/multirobotsim_dcenlocal.py, utils/metrics.py, graphs/losses/*) from the reference checkout, unmodified,
 either against the reference's own model or against this repo's drop-in modules.
 
-Build container only (the GPU box has no /root/reference).  Used by
+Needs a reference checkout (GNNPP_REFERENCE_ROOT); only the golden-data generators use it.  Used by
   * tests/golden/make_agent_trace.py   reference agent + reference model  -> tests/golden/agent_trace.npz
   * tests/test_reference_agent_dropin.py   reference agent + gnn_pathplanning_b200.install_dropin()
 
@@ -26,7 +26,7 @@ import types
 import numpy as np
 import torch
 
-REF_ROOT = os.environ.get("GNNPP_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("GNNPP_REFERENCE_ROOT", "")
 STUBBED = ("matplotlib", "seaborn", "tensorboardX", "easydict", "torchsummaryX", "hashids", "skimage", "drawSvg",
            "plotly", "mpl_toolkits")
 REF_PACKAGES = ("agents", "utils", "graphs", "dataloader", "onlineExpert", "offlineExpert")

@@ -1,12 +1,12 @@
-"""TEST INFRASTRUCTURE ONLY -- import the *unmodified* reference from /root/reference.
+"""TEST INFRASTRUCTURE ONLY -- import the *unmodified* reference from the reference checkout.
 
-Only usable inside the build container (the GPU box has no /root/reference).
+Needs a reference checkout (GNNPP_REFERENCE_ROOT); only the golden-data generators use it.
 Used by tests/golden/make_golden.py to generate the committed golden vectors and
-by the container-only tests that pin oracle/planner_oracle.py against the real
+by tests/golden/make_reference_cases.py, whose output pins oracle/planner_oracle.py against the real
 reference code.  Nothing here is imported by the product package.
 
 Why a shim is needed (SURVEY.md section 8c):
-  * /root/reference/utils/__init__.py and graphs/__init__.py eagerly import every
+  * gnn_pathplanning/utils/__init__.py and graphs/__init__.py eagerly import every
     sibling module (matplotlib, easydict, tensorboardX ... absent here), so the
     packages are pre-registered as bare namespace modules whose __path__ points
     into the reference tree and whose __init__ therefore never runs.
@@ -17,7 +17,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("GNNPP_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("GNNPP_REFERENCE_ROOT", "")
 
 
 def available() -> bool:

@@ -4,14 +4,14 @@ Restatement (numpy / plain Python, one episode, sequential) of the part of the r
 surrounds the planner's forward every step -- the checker for gnn_pathplanning_b200/csrc/rollout.cu (SURVEY.md
 section 8 rows f1 / f2):
 
-    multiRobotSim.getCurrentState    /root/reference/utils/multirobotsim_dcenlocal.py:425-453
-      -> AgentState.toInputTensor    /root/reference/dataloader/statetransformer.py:82-130 (projected goal :47-66)
-    multiRobotSim.getGSO             /root/reference/utils/multirobotsim_dcenlocal.py:367-394
-      -> computeAdjacencyMatrix      :320-365, isConnected /root/reference/utils/graphUtils/graphTools.py:396-423
+    multiRobotSim.getCurrentState    gnn_pathplanning/utils/multirobotsim_dcenlocal.py:425-453
+      -> AgentState.toInputTensor    gnn_pathplanning/dataloader/statetransformer.py:82-130 (projected goal :47-66)
+    multiRobotSim.getGSO             gnn_pathplanning/utils/multirobotsim_dcenlocal.py:367-394
+      -> computeAdjacencyMatrix      :320-365, isConnected gnn_pathplanning/utils/graphUtils/graphTools.py:396-423
     multiRobotSim.move               :562-723, interRobotCollision :462-555
 
 PARITY PINNING: tests/test_sim_oracle_vs_reference.py runs this class and the reference's own multiRobotSim side by side
-in the build container (same cases, same logits, `random.choice` replaced on both sides by the round-robin rule below);
+by tests/golden/make_reference_cases.py (same cases, same logits, `random.choice` replaced on both sides by the round-robin rule below);
 tests/golden/make_rollout_trace.py records reference rollouts into tests/golden/rollout_trace.npz, which
 tests/test_oracle_golden.py (CPU) and tests/test_gpu_rollout.py (GPU) replay.
 

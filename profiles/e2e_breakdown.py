@@ -1,7 +1,7 @@
 """Host-side cost of the pipelined host-buffer path at the headline size: time spent in infer_host_async
 (submission) and in wait() per step, next to the device-only step time."""
 import sys, time
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 import torch
 import gnn_pathplanning_b200 as gp
 from gnn_pathplanning_b200 import synthetic

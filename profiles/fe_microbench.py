@@ -52,5 +52,5 @@ for B in sizes:
             _lib.check(nat.lib.gpp_planner_set_profiling(nat.handle, 0))
         fe_us = fe_ms.value * 1e3 / max(1, nst.value)
         print("agents=%6d  feature=%-4s  feature kernel %9.1f us (%6.0f cycles/agent/SM-slot)  filter %7.1f us  step %9.1f us  %7.2f M agent-steps/s"
-              % (B * N, fe, fe_us, fe_us * 1965.0 / max(1.0, B * N / 148.0), gf_ms.value * 1e3 / max(1, nst.value), step_us,
+              % (B * N, fe, fe_us, fe_us * 1980.0 / max(1.0, B * N / torch.cuda.get_device_properties(0).multi_processor_count), gf_ms.value * 1e3 / max(1, nst.value), step_us,
                  B * N / step_us), flush=True)

@@ -1,6 +1,6 @@
-"""Graph-filter kernel micro-benchmark (device-resident, CUDA events): CUDA-core vs tcgen05 kernel over
+"""Graph-filter kernel micro-benchmark (device-resident, CUDA events): CUDA-core vs tensor-core (wgmma) kernels over
 batch sizes, reported as agent-steps/s and as algorithmic GB/s (SURVEY.md 8d: 4*(G+N+F) bytes per
-agent-step) against the measured HBM peak.  usage: python profiles/gf_microbench.py [N] [K] [modes, e.g. 3 or 1,2,3]"""
+agent-step) against the measured HBM peak (else the H100 SXM data-sheet figure).  usage: python profiles/gf_microbench.py [N] [K] [modes, e.g. 3 or 1,2,3]"""
 import json
 import os
 import subprocess
@@ -46,9 +46,9 @@ if __name__ == "__main__":
     N = int(sys.argv[1]) if len(sys.argv) > 1 else 10
     K = int(sys.argv[2]) if len(sys.argv) > 2 else 3
     peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
-        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0     # H100 SXM data sheet, HBM3
     modes = [int(m) for m in sys.argv[3].split(",")] if len(sys.argv) > 3 else [1, 2, 3]
-    for mode, name in ((1, "cuda-core"), (2, "tcgen05-tf32"), (3, "tcgen05-pair")):
+    for mode, name in ((1, "cuda-core"), (2, "wgmma-3xtf32"), (3, "wgmma-pair")):
         if mode not in modes:
             continue
         r = subprocess.run([sys.executable, "-c", CHILD % ROOT, str(N), str(K), str(mode)], capture_output=True, text=True)

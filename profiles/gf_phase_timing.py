@@ -1,7 +1,7 @@
 """Per-phase cycles of block 0 of feature_kernel and gf_fwd_kernel inside the planner forward
 ("fe_timing" / "gf_timing" debug options)."""
 import os, sys, ctypes as C
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 import torch
 import gnn_pathplanning_b200 as gp
 from gnn_pathplanning_b200 import _lib, synthetic

@@ -31,5 +31,5 @@ for mask in (0, 1, 2, 3, 4, 7, 8, 15):
     e1.record()
     torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 1e3 / 5
-    print("ablate %2d  %-36s %8.1f us   %.3f us per tile per CTA" % (mask, names[mask], us, us / (B / 12 / 148)))
+    print("ablate %2d  %-36s %8.1f us   %.3f us per tile per CTA" % (mask, names[mask], us, us / (B / 12 / torch.cuda.get_device_properties(0).multi_processor_count)))
 _lib.set_debug_option("pair_ablate", 0)

@@ -1,6 +1,6 @@
 """A few planner forwards (for ncu captures).  usage: run_planner_once.py [B N gf_mode fe_mode]"""
 import sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 import torch
 import gnn_pathplanning_b200 as gp
 from gnn_pathplanning_b200 import synthetic

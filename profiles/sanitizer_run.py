@@ -1,5 +1,5 @@
 import sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 import numpy as np, torch
 import gnn_pathplanning_b200 as gp
 from gnn_pathplanning_b200 import synthetic

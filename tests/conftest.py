@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -37,8 +37,29 @@ def rel_err(a, ref):
     return float(np.abs(a - ref).max()) / denom
 
 
+class GoldenRecord:
+    """One golden record: `name.npz` merged with its `name.partN.npz` parts (tests/golden/golden_io.py)."""
+
+    def __init__(self, name):
+        stem = name[:-4]
+        paths = [os.path.join(GOLDEN, name)]
+        i = 1
+        while os.path.isfile(os.path.join(GOLDEN, "%s.part%d.npz" % (stem, i))):
+            paths.append(os.path.join(GOLDEN, "%s.part%d.npz" % (stem, i)))
+            i += 1
+        self._arrays = {}
+        for p in paths:
+            with np.load(p, allow_pickle=False) as z:
+                self._arrays.update({k: z[k] for k in z.files})
+        self.files = list(self._arrays)
+
+    def __getitem__(self, key):
+        return self._arrays[key]
+
+    def __contains__(self, key):
+        return key in self._arrays
+
+
 @pytest.fixture(scope="session")
 def golden():
-    def load(name):
-        return np.load(os.path.join(GOLDEN, name), allow_pickle=False)
-    return load
+    return GoldenRecord

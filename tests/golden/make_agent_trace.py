@@ -2,9 +2,8 @@
 (agents/decentralplannerlocal.py: train_one_epoch :276-326 on one batch, then one rollout case through
 mutliAgent_ActionPolicy :535-648 with the real simulator) against the reference's own model on CPU.
 
-Build container only:   python tests/golden/make_agent_trace.py
-Consumed by tests/test_reference_agent_dropin.py (CPU: the same agent code against install_dropin())
-and tests/test_gpu_agent_trace.py (GPU: the recorded calls replayed on the CUDA module).
+Run with a reference checkout:   GNNPP_REFERENCE_ROOT=<checkout> python tests/golden/make_agent_trace.py
+Consumed by tests/test_gpu_agent_trace.py (GPU: the recorded calls replayed on the CUDA module).
 """
 import os
 import sys
@@ -17,7 +16,9 @@ warnings.filterwarnings("ignore")
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
+import golden_io  # noqa: E402
 from oracle import ref_agent  # noqa: E402
 from oracle import planner_oracle as po  # noqa: E402
 from gnn_pathplanning_b200 import synthetic  # noqa: E402
@@ -56,7 +57,7 @@ def main():
                 "case_map": case[3].numpy()})
     out.update(tr)
     path = os.path.join(HERE, "agent_trace.npz")
-    np.savez_compressed(path, **out)
+    golden_io.savez_split(path, dict(out))
     print("wrote", path, "rollout steps:", tr["rollout_x"].shape[0], "train loss %.6f" % tr["train_loss"],
           "all_reach_goal", int(tr["all_reach_goal"]))
 

@@ -1,9 +1,9 @@
 """Generates the committed golden vectors by running the UNMODIFIED reference
-(/root/reference, imported through oracle/ref_shim.py) on CPU.
+(the reference checkout, imported through oracle/ref_shim.py) on CPU.
 
-Run in the build container only:   python tests/golden/make_golden.py
+Run with a reference checkout:   GNNPP_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py
 Outputs (float32 unless noted), all consumed by tests/test_oracle_golden.py (CPU,
-pins the oracle) and tests/test_gpu_parity.py (GPU, pins the CUDA path):
+pins the oracle) and tests/test_gpu_*.py (GPU tests, pin the CUDA path):
 
   rnn_cases.npz       GraphFilterRNNBatch / GraphFilterMoRNNBatch / GraphFilterL2ShareBatch, two recurrent steps
   gf_cases.npz        GraphFilterBatch / BatchLSIGF: hand-derivable KATs (SURVEY 8c)
@@ -27,7 +27,9 @@ warnings.filterwarnings("ignore")
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
+import golden_io  # noqa: E402
 from oracle import ref_shim  # noqa: E402
 from oracle import planner_oracle as po  # noqa: E402
 from gnn_pathplanning_b200 import synthetic  # noqa: E402
@@ -209,11 +211,11 @@ def input_cases(st, sim):
 def main():
     gml, dcp, st = ref_shim.load()
     sim = ref_shim.load_sim()
-    np.savez_compressed(os.path.join(HERE, "gf_cases.npz"), **gf_cases(gml))
-    np.savez_compressed(os.path.join(HERE, "rnn_cases.npz"), **rnn_cases(gml))
-    np.savez_compressed(os.path.join(HERE, "planner_K3.npz"), **planner_case(dcp, 3, 10, 4, 20, False))
-    np.savez_compressed(os.path.join(HERE, "planner_K2.npz"), **planner_case(dcp, 2, 10, 1, 20, True))
-    np.savez_compressed(os.path.join(HERE, "inputs.npz"), **input_cases(st, sim))
+    golden_io.savez_split(os.path.join(HERE, "gf_cases.npz"), gf_cases(gml))
+    golden_io.savez_split(os.path.join(HERE, "rnn_cases.npz"), rnn_cases(gml))
+    golden_io.savez_split(os.path.join(HERE, "planner_K3.npz"), planner_case(dcp, 3, 10, 4, 20, False))
+    golden_io.savez_split(os.path.join(HERE, "planner_K2.npz"), planner_case(dcp, 2, 10, 1, 20, True))
+    golden_io.savez_split(os.path.join(HERE, "inputs.npz"), input_cases(st, sim))
     for f in sorted(os.listdir(HERE)):
         if f.endswith(".npz"):
             print(f, os.path.getsize(os.path.join(HERE, f)))

@@ -1,7 +1,7 @@
 """Generates tests/golden/rollout_trace.npz: rollouts of the reference's own simulator
 (utils/multirobotsim_dcenlocal.py, unmodified; `random.choice` = the round-robin contract, oracle/ref_sim.py) under a
 seeded goal-seeking policy -- per step the FOV tensor and float64 GSO the simulator built, the logits it was fed, and
-the positions / actions / flags it produced.  Build container only:   python tests/golden/make_rollout_trace.py
+the positions / actions / flags it produced.  Run with a reference checkout:   GNNPP_REFERENCE_ROOT=<checkout> python tests/golden/make_rollout_trace.py
 Consumed by tests/test_oracle_golden.py (CPU: oracle/sim_oracle.py) and tests/test_gpu_rollout.py (GPU: rollout.cu)."""
 import os
 import sys
@@ -13,7 +13,9 @@ warnings.filterwarnings("ignore")
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
+import golden_io  # noqa: E402
 from oracle import ref_agent, ref_sim  # noqa: E402
 
 SETS = {  # name: (N, W, density, makespan, steps, episodes, policy noise)
@@ -41,7 +43,7 @@ def main():
             print(name, "N=%d W=%d T=%d episodes=%d: %d moves, %d tie-break draws, %d episodes finished" % (
                 N, W, T, E, moved, sum(int(t["choices"]) for t in traces), sum(int(t["flags"][:, 0].any()) for t in traces)))
     path = os.path.join(HERE, "rollout_trace.npz")
-    np.savez_compressed(path, **out)
+    golden_io.savez_split(path, dict(out))
     print("wrote", path, os.path.getsize(path))
 
 

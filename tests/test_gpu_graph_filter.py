@@ -127,7 +127,7 @@ def test_zero_padding_path_and_asserts():
 def test_properties_at_full_size():
     """BASELINE config 4 size (N=40, B=256 -> 10,240 node rows): the CPU oracle at the full size in both
     layouts (feature-major = the reference API, CUDA-core kernel; node-major = the planner-internal layout, which
-    the automatic choice routes to the tcgen05 kernel at this size), then size-independent properties: linearity
+    the automatic choice routes to the tensor-core kernel at this size), then size-independent properties: linearity
     in x, K=1 reduces to a per-node linear map, identity GSO collapses the taps, permutation equivariance."""
     import gnn_pathplanning_b200 as g
     from oracle import planner_oracle as po

@@ -1,5 +1,5 @@
-"""GPU parity of the CTA-pair tcgen05 graph filter (gf_fwd_pair_kernel: propagate in registers, 2-way fp16 split with
-per-sample power-of-two scaling, cta_group::2 MMAs with the taps resident in shared memory, TMA tensor stores)
+"""GPU parity of the fp16-split pair graph filter (gf_fwd_pair_kernel: propagate in registers, 2-way fp16 split with
+per-sample power-of-two scaling, wgmma with the taps streamed through a bulk-copy ring)
 against the CPU oracle: standalone op through the C ABI, and inside the planner (fused ReLU + action MLP)."""
 import numpy as np
 import pytest

@@ -97,7 +97,7 @@ def test_eval_vs_oracle(N, K, B, map_w):
 
 
 def test_repeated_calls_with_changing_batch_sizes():
-    """One handle, many launches: the filter kernel changes with the batch size (small-batch tcgen05 clusters below
+    """One handle, many launches: the filter kernel changes with the batch size (small-batch wgmma clusters below
     4,096 node rows, the CTA-pair kernel above) and the per-handle scratch is regrown when the batch grows."""
     from gnn_pathplanning_b200 import synthetic
     from oracle import planner_oracle as po
@@ -256,7 +256,7 @@ def test_train_step_vs_fp64_oracle_at_config_sizes(N, K, B, map_w):
 
 def test_full_c4_eval_vs_oracle():
     """BASELINE config 4 at FULL size: K=3, 40 agents, 50x50 map, batch 256 (10,240 node rows: the automatic
-    choice routes the graph filter to the tcgen05 kernel); the forced tcgen05 and CUDA-core filters as well."""
+    choice routes the graph filter to the tensor-core kernel); the forced tensor-core and CUDA-core filters as well."""
     from gnn_pathplanning_b200 import synthetic
     from oracle import planner_oracle as po
     N, K, B, map_w = 40, 3, 256, 50

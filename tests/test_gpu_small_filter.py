@@ -1,8 +1,8 @@
-"""GPU parity of the small-batch tcgen05 graph filter (gf_small_mma_kernel: N = 10, K <= 3, below 4,096 node rows --
+"""GPU parity of the small-batch wgmma graph filter (gf_small_mma_kernel: N = 10, K <= 3, below 4,096 node rows --
 the filter of the benchmark configuration and of rollout steps) through the planner's C ABI: against the CPU oracle
 and against the CUDA-core kernel of the same library, at ragged tile counts, float64 GSOs, signed / badly scaled
 GSOs (per-sample power-of-two scaling), isolated agents and the largest batch the kernel takes.
-Reference: /root/reference/utils/graphUtils/graphML.py:2342-2366, graphs/models/decentralplanner.py:284-318."""
+Reference: gnn_pathplanning/utils/graphUtils/graphML.py:2342-2366, graphs/models/decentralplanner.py:284-318."""
 import numpy as np
 import pytest
 import torch

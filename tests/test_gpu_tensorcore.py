@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (3xTF32, TMEM accumulator) graph-filter path -- plumbing self-test, then parity
+"""GPU: the wgmma (3xTF32, register accumulator) graph-filter path -- plumbing self-test, then parity
 of the planner with the tensor-core filter kernel against the CPU oracle and the golden vectors."""
 import ctypes as C
 
@@ -46,7 +46,7 @@ def _model(sd, N, K, mode, fe_mode="cuda"):
 @pytest.mark.parametrize("N,K,B,map_w", [(10, 3, 64, 20), (10, 3, 1, 20), (7, 2, 3, 12), (20, 3, 40, 28), (40, 3, 7, 50),
                                          (1, 3, 9, 8), (10, 3, 500, 20), (3, 1, 101, 12)])
 def test_planner_tc_feature_extractor_vs_oracle(N, K, B, map_w):
-    """tcgen05 implicit-GEMM CNN + compress MLP (feature_tc_kernel) against the CPU oracle."""
+    """wgmma implicit-GEMM CNN + compress MLP (feature_tc_kernel) against the CPU oracle."""
     from gnn_pathplanning_b200 import synthetic
     from oracle import planner_oracle as po
     sd = po.init_state_dict(K, seed=N + K + 1)
@@ -117,7 +117,7 @@ def test_tc_mode_rejects_oversized_graphs():
 @pytest.mark.parametrize("N,K,B,map_w", [(10, 3, 64, 20), (10, 3, 1, 20), (7, 2, 3, 12), (20, 3, 40, 28), (40, 3, 7, 50),
                                          (1, 3, 9, 8), (10, 3, 500, 20), (3, 1, 101, 12), (10, 3, 4000, 20)])
 def test_planner_mma_feature_extractor_vs_oracle(N, K, B, map_w):
-    """im2col-free fp16-split tcgen05 CNN + compress MLP (feature_mma_kernel) against the CPU oracle, features and
+    """im2col-free fp16-split wgmma CNN + compress MLP (feature_mma_kernel) against the CPU oracle, features and
     logits, incl. ragged last tiles (B*N not a multiple of 8) and several tiles per CTA (40,000 agents)."""
     from gnn_pathplanning_b200 import synthetic
     from oracle import planner_oracle as po

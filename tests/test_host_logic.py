@@ -79,7 +79,7 @@ def test_planner_api_asserts_on_cpu():
 
 def test_dropin_hook_routes_three_names_and_nothing_else(tmp_path):
     """install_dropin() on a stand-in tree laid out like the reference (package __init__s that eagerly import
-    every sibling module, as /root/reference/utils/__init__.py:6-10 does): the three hot-path module names
+    every sibling module, as gnn_pathplanning/utils/__init__.py:6-10 does): the three hot-path module names
     resolve to this package, every other module of the same packages still comes from the tree."""
     import gnn_pathplanning_b200 as gp
     import sys
