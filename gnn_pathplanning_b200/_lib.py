@@ -29,6 +29,10 @@ GPP_ERR_INVALID = -1
 GPP_ERR_UNSUPPORTED = -2
 FEATURE_MAJOR = 0   # [B, G, N]  (reference API layout)
 NODE_MAJOR = 1      # [B, N, G]
+# columns of gpp_rollout_record's outcome rows, in the order of gpp_outcome_field (include/gnnpp_b200.h)
+OUTCOME_FIELDS = ("steps", "all_reach_goal", "no_reach_goal_sh", "find_optimal", "collision_free", "collision_predicted",
+                  "collision_happened", "num_reach_goal", "makespan_predict", "makespan_target", "flowtime_predict",
+                  "flowtime_target", "valid")
 
 # every symbol include/gnnpp_b200.h declares
 EXPORTED = (
@@ -38,6 +42,7 @@ EXPORTED = (
     "gpp_planner_create", "gpp_planner_destroy", "gpp_planner_set_weights",
     "gpp_planner_forward", "gpp_planner_forward_host",
     "gpp_planner_train_workspace_bytes", "gpp_planner_train_forward", "gpp_planner_train_backward", "gpp_planner_ce_loss", "gpp_rollout_build_inputs", "gpp_rollout_move",
+    "gpp_rollout_expert_metrics", "gpp_rollout_record",
     "gpp_planner_forward_host_async", "gpp_planner_wait", "gpp_planner_forward_async", "gpp_planner_join",
     "gpp_planner_set_profiling", "gpp_planner_get_profile",
     "gpp_planner_set_graph_filter_mode", "gpp_planner_set_feature_mode",
@@ -181,6 +186,10 @@ def load():
         lib.gpp_rollout_build_inputs.argtypes = [vp, vp, vp, i, vp, i, vp, vp, i, vp, i, i, i, vp]
         lib.gpp_rollout_move.restype = i
         lib.gpp_rollout_move.argtypes = [vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, i, i, i, i, vp]
+        lib.gpp_rollout_expert_metrics.restype = i
+        lib.gpp_rollout_expert_metrics.argtypes = [vp, vp, vp, i, vp, vp, vp, i, i, vp]
+        lib.gpp_rollout_record.restype = i
+        lib.gpp_rollout_record.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i, i, i, vp]
         lib.gpp_planner_forward_host_async.restype = i
         lib.gpp_planner_forward_host_async.argtypes = [vp, vp, vp, i, vp, i, i, C.POINTER(C.c_ulonglong)]
         lib.gpp_planner_wait.restype = i

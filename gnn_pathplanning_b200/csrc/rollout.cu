@@ -10,6 +10,8 @@
 // integer agent positions that never leave the device; rollout_move_kernel turns the planner's logits into moves with the
 // reference's edge / obstacle / inter-robot collision shielding.  Both are integer / IEEE-double restatements of the
 // reference's arithmetic: bit-exact by construction (tests/test_gpu_rollout.py).
+#include <climits>
+
 #include "common.cuh"
 
 namespace gpp {
@@ -400,6 +402,152 @@ __global__ void __launch_bounds__(128) rollout_move_warp_kernel(const RoMoveArgs
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Evaluation bookkeeping (the scoring half of agents/decentralplannerlocal.py:535-648).  Both kernels run one warp per
+// episode; agent i lives on lane i % 32 (two agents per lane for 32 < N <= 64) and reductions over agents are shuffles.
+// ---------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ int ro_warp_max(int v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ int ro_warp_min(int v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ int ro_warp_sum(int v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+struct RoExpertArgs {
+    const int* start;      // [B][N][2]
+    const int* goal;       // [B][N][2]
+    const int* action;     // [B][N][T] expert action indices (0..4)
+    int* makespan;         // [B] out
+    int* flowtime;         // [B] out
+    int* valid;            // [B] out
+    int B, N, T;
+};
+
+// multiRobotSim.getPathTarget (utils/multirobotsim_dcenlocal.py:159-230): every agent replays its expert actions from
+// its start for all T steps, ignoring obstacles and the other agents.  startStep = first step whose action is not stop,
+// endStep = step + 1 at the first arrival on the goal.  The targets exist only if every agent arrives (else the
+// reference keeps 0 and later divides by it, utils/metrics.py:110-111) and every arriving agent has moved (else it
+// computes end - None); an action outside 0..4 is an IndexError there.  Unusable targets are written as 0.
+__global__ void __launch_bounds__(128) rollout_expert_kernel(const RoExpertArgs a) {
+    const int b = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (b >= a.B) return;
+    const int N = a.N, T = a.T;
+    int end_max = INT_MIN, start_min = INT_MAX, flow = 0, bad = 0;
+    for (int i = lane; i < N; i += 32) {
+        const int* st = a.start + ((size_t)b * N + i) * 2;
+        const int* gl = a.goal + ((size_t)b * N + i) * 2;
+        const int* act = a.action + ((size_t)b * N + i) * T;
+        int x = st[0], y = st[1], sst = -1, est = -1;
+        const int gx = gl[0], gy = gl[1];
+        for (int t = 0; t < T; ++t) {
+            const int k = act[t];
+            if (k < 0 || k > 4) { bad = 1; break; }
+            if (k != 4 && sst < 0) sst = t;
+            x += k == 0 ? -1 : k == 2 ? 1 : 0;
+            y += k == 1 ? -1 : k == 3 ? 1 : 0;
+            if (est < 0 && x == gx && y == gy) est = t + 1;
+        }
+        bad |= est < 0 || sst < 0;
+        end_max = max(end_max, est);
+        start_min = min(start_min, sst);
+        flow += est - sst;
+    }
+    end_max = ro_warp_max(end_max);
+    start_min = ro_warp_min(start_min);
+    flow = ro_warp_sum(flow);
+    bad = ro_warp_max(bad);
+    const int makespan = end_max - start_min;
+    const bool ok = !bad && makespan != 0 && flow != 0;
+    if (lane == 0) {
+        a.makespan[b] = ok ? makespan : 0;
+        a.flowtime[b] = ok ? flow : 0;
+        a.valid[b] = ok;
+    }
+}
+
+struct RoRecordArgs {
+    const int* flags;            // [B][3] of the move just made
+    const int* maxstep;          // [B]
+    const int* reached;          // [B][N]
+    const int* start_step;       // [B][N]
+    const int* end_step;         // [B][N]
+    const int* makespan_target;  // [B] or null
+    const int* flowtime_target;  // [B] (read only with makespan_target)
+    int* active;                 // [B] in / out
+    int* outcome;                // [B][GPP_OUTCOME_FIELDS] in / out
+    int B, N, currentstep;
+};
+
+// One step of mutliAgent_ActionPolicy's bookkeeping (agents/decentralplannerlocal.py:555-624) after the move of step
+// `currentstep`.  Episodes that were not moved (active == 0) keep their record: their flags are stale.
+__global__ void __launch_bounds__(128) rollout_record_kernel(const RoRecordArgs a) {
+    const int b = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (b >= a.B) return;
+    if (!a.active[b]) return;
+    const int N = a.N, step = a.currentstep, maxstep = a.maxstep[b];
+    int* out = a.outcome + (size_t)b * GPP_OUTCOME_FIELDS;
+    const bool all_reach = a.flags[3 * b] != 0;
+    const bool happened = out[GPP_OUTCOME_COLLISION_HAPPENED] || a.flags[3 * b + 1];    // :593-594
+    const bool predicted = out[GPP_OUTCOME_COLLISION_PREDICTED] || a.flags[3 * b + 2];  // :597-598
+    const bool timeout = step >= maxstep;
+    const bool done = all_reach || timeout;                                             // :600-606
+    if (!done) {
+        if (lane == 0) {
+            out[GPP_OUTCOME_STEPS] = step;
+            out[GPP_OUTCOME_COLLISION_HAPPENED] = happened;
+            out[GPP_OUTCOME_COLLISION_PREDICTED] = predicted;
+        }
+        return;
+    }
+    // the move of the last step computed the predicted makespan / flowtime (multirobotsim_dcenlocal.py:693-715)
+    int end_max = INT_MIN, start_min = INT_MAX, flow = 0, n_reach = 0, undefined = 0;
+    for (int i = lane; i < N; i += 32) {
+        const int sst = a.start_step[(size_t)b * N + i], est = a.end_step[(size_t)b * N + i];
+        undefined |= sst < 0 || est < 0;          // end - None: the reference raises TypeError
+        end_max = max(end_max, est);
+        start_min = min(start_min, sst);
+        flow += est - sst;
+        n_reach += a.reached[(size_t)b * N + i] != 0;
+    }
+    end_max = ro_warp_max(end_max);
+    start_min = ro_warp_min(start_min);
+    flow = ro_warp_sum(flow);
+    n_reach = ro_warp_sum(n_reach);
+    undefined = ro_warp_max(undefined);
+    if (lane != 0) return;
+    const bool has_target = a.makespan_target != nullptr;
+    const int mt = has_target ? a.makespan_target[b] : 0, ft = has_target ? a.flowtime_target[b] : 0;
+    const bool collision_free = all_reach && !happened;                                 // :611-612
+    // compare_makespan / compare_flowtime keep getOptimalityMetrics' pre-loop defaults (:555, multirobotsim :91-92)
+    // unless checkOptimality runs (:614, :619, :622)
+    const bool checked = collision_free || timeout;
+    const bool optimal = has_target && collision_free && !timeout && end_max - start_min <= mt && flow <= ft;
+    out[GPP_OUTCOME_STEPS] = step;
+    out[GPP_OUTCOME_ALL_REACH_GOAL] = all_reach;
+    out[GPP_OUTCOME_NO_REACH_GOAL_SH] = timeout && !all_reach && predicted && !happened;          // :621-624
+    out[GPP_OUTCOME_FIND_OPTIMAL] = optimal;
+    out[GPP_OUTCOME_COLLISION_FREE] = collision_free;
+    out[GPP_OUTCOME_COLLISION_PREDICTED] = predicted;
+    out[GPP_OUTCOME_COLLISION_HAPPENED] = happened;
+    out[GPP_OUTCOME_NUM_REACH_GOAL] = n_reach;
+    out[GPP_OUTCOME_MAKESPAN_PREDICT] = checked ? end_max - start_min : maxstep;
+    out[GPP_OUTCOME_MAKESPAN_TARGET] = mt;
+    out[GPP_OUTCOME_FLOWTIME_PREDICT] = checked ? flow : maxstep * N;
+    out[GPP_OUTCOME_FLOWTIME_TARGET] = ft;
+    // the reference scores this case without raising: predicted steps defined, targets usable (nonzero divisors)
+    out[GPP_OUTCOME_VALID] = !undefined && (!has_target || (mt != 0 && ft != 0));
+    a.active[b] = 0;
+}
+
 }  // namespace gpp
 
 using namespace gpp;
@@ -440,6 +588,42 @@ extern "C" int gpp_rollout_move(const float* logits, int* pos, const int* goal, 
         rollout_move_warp_kernel<<<(B + 3) / 4, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     else
         rollout_move_kernel<<<(B + 63) / 64, 64, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+    GPP_LAUNCH_CHECK();
+    return GPP_OK;
+}
+
+extern "C" int gpp_rollout_expert_metrics(const int* start, const int* goal, const int* expert_action, int T,
+                                          int* makespan_target, int* flowtime_target, int* target_valid, int B, int N,
+                                          void* stream) {
+    GPP_REQUIRE(start && goal && expert_action && makespan_target && flowtime_target && target_valid, GPP_ERR_INVALID,
+                "rollout_expert_metrics: null pointer");
+    GPP_REQUIRE(B >= 0 && N >= 1 && T >= 1, GPP_ERR_INVALID, "rollout_expert_metrics: bad sizes B=%d N=%d T=%d", B, N, T);
+    GPP_REQUIRE(N <= RO_MAX_N, GPP_ERR_UNSUPPORTED, "rollout_expert_metrics: N=%d > %d agents", N, RO_MAX_N);
+    if (B == 0) return GPP_OK;
+    RoExpertArgs a;
+    a.start = start; a.goal = goal; a.action = expert_action;
+    a.makespan = makespan_target; a.flowtime = flowtime_target; a.valid = target_valid;
+    a.B = B; a.N = N; a.T = T;
+    rollout_expert_kernel<<<(B + 3) / 4, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+    GPP_LAUNCH_CHECK();
+    return GPP_OK;
+}
+
+extern "C" int gpp_rollout_record(const int* flags, const int* maxstep, const int* reached, const int* start_step,
+                                  const int* end_step, const int* makespan_target, const int* flowtime_target,
+                                  int* active, int* outcome, int currentstep, int B, int N, void* stream) {
+    GPP_REQUIRE(flags && maxstep && reached && start_step && end_step && active && outcome &&
+                    (!makespan_target || flowtime_target),
+                GPP_ERR_INVALID, "rollout_record: null pointer");
+    GPP_REQUIRE(B >= 0 && N >= 1 && currentstep >= 1, GPP_ERR_INVALID, "rollout_record: bad sizes B=%d N=%d step=%d",
+                B, N, currentstep);
+    GPP_REQUIRE(N <= RO_MAX_N, GPP_ERR_UNSUPPORTED, "rollout_record: N=%d > %d agents", N, RO_MAX_N);
+    if (B == 0) return GPP_OK;
+    RoRecordArgs a;
+    a.flags = flags; a.maxstep = maxstep; a.reached = reached; a.start_step = start_step; a.end_step = end_step;
+    a.makespan_target = makespan_target; a.flowtime_target = flowtime_target; a.active = active; a.outcome = outcome;
+    a.B = B; a.N = N; a.currentstep = currentstep;
+    rollout_record_kernel<<<(B + 3) / 4, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     GPP_LAUNCH_CHECK();
     return GPP_OK;
 }

@@ -4,8 +4,10 @@ The reference rolls ONE episode at a time on the host (agents/decentralplannerlo
 the field-of-view tensor and the graph shift operator with numpy / scipy (`multiRobotSim.getCurrentState`, `.getGSO`),
 copies them to the device, runs the model, pulls N tiny argmax results back and moves the agents in Python dicts
 (`multiRobotSim.move`).  `BatchedRollout` keeps B episodes on the device and advances them in lock-step: positions never
-leave HBM, the per-step work is three library launches (inputs, planner forward, move) and there is no per-step
-host <-> device copy -- only the `done` flags are read back every `poll_every` steps.
+leave HBM, the per-step work is four library launches (inputs, planner forward, move, outcome record) and there is no
+per-step host <-> device copy -- only the `done` flags are read back every `poll_every` steps.  With expert actions
+given to `setup`, `outcome()` is what `mutliAgent_ActionPolicy` returns per case; `gnn_pathplanning_b200.evaluate`
+turns a test loader into these batched rollouts and the reference's metrics.
 
 Mirrors the simulator's interface where it has one: `setup`, `getCurrentState`, `getGSO`, `move`, `getMaxstep`,
 `count_numAgents_ReachGoal`, plus `run(model)` for the whole loop.  The only behavioural difference is the documented
@@ -27,9 +29,10 @@ class BatchedRollout:
         self.B = 0
 
     # ------------------------------------------------------------------ setup (multirobotsim_dcenlocal.py:54-143)
-    def setup(self, start, goal, maps, maxstep):
+    def setup(self, start, goal, maps, maxstep, expert_actions=None):
         """start, goal: [B,N,2] integer cells; maps: [B,W,W] or [W,W] {0,1}; maxstep: int or [B]
-        (the reference: makespanTarget * rate_maxstep, :76-81)."""
+        (the reference: makespanTarget * rate_maxstep, :76-81); expert_actions: optional [B,N,T] expert action
+        indices, replayed once into the target makespan / flowtime of every episode (getPathTarget, :159-230)."""
         dev = self.device
         self.pos = torch.as_tensor(start).to(dev, torch.int32).contiguous().clone()
         self.goal = torch.as_tensor(goal).to(dev, torch.int32).contiguous()
@@ -54,6 +57,19 @@ class BatchedRollout:
         self.connected = torch.zeros(B, device=dev, dtype=torch.int32)
         self.x = torch.empty(B, N, 3, 11, 11, device=dev, dtype=torch.float32)
         self.S = torch.empty(B, N, N, device=dev, dtype=torch.float64)
+        self.outcome_rows = torch.zeros(B, len(_lib.OUTCOME_FIELDS), device=dev, dtype=torch.int32)
+        self.makespan_target = self.flowtime_target = self.target_valid = None
+        if expert_actions is not None:
+            act = torch.as_tensor(expert_actions).to(dev, torch.int32).contiguous()
+            assert act.dim() == 3 and tuple(act.shape[:2]) == (B, N)
+            self.makespan_target = torch.zeros(B, device=dev, dtype=torch.int32)
+            self.flowtime_target = torch.zeros(B, device=dev, dtype=torch.int32)
+            self.target_valid = torch.zeros(B, device=dev, dtype=torch.int32)
+            with torch.cuda.device(dev):
+                _lib.check(self.lib.gpp_rollout_expert_metrics(
+                    self.pos.data_ptr(), self.goal.data_ptr(), act.data_ptr(), int(act.shape[2]),
+                    self.makespan_target.data_ptr(), self.flowtime_target.data_ptr(), self.target_valid.data_ptr(),
+                    B, N, self._stream()))
         self.step = 0
         return self
 
@@ -99,11 +115,30 @@ class BatchedRollout:
     def count_numAgents_ReachGoal(self):
         return self.reached.sum(dim=1)
 
+    # ------------------------------------------------------------------ per-episode outcome (agents/...local.py:555-624)
+    def record(self, currentstep: int):
+        """Folds the flags of the move of `currentstep` into each still-active episode's outcome record; an episode
+        whose loop the reference would leave now (all agents had reached their goals, or maxstep) gets its final
+        outcome and is marked inactive."""
+        has_target = self.makespan_target is not None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.gpp_rollout_record(
+                self.flags.data_ptr(), self.maxstep.data_ptr(), self.reached.data_ptr(), self.start_step.data_ptr(),
+                self.end_step.data_ptr(), self.makespan_target.data_ptr() if has_target else None,
+                self.flowtime_target.data_ptr() if has_target else None, self.active.data_ptr(),
+                self.outcome_rows.data_ptr(), int(currentstep), self.B, self.N, self._stream()))
+
+    def outcome(self):
+        """The per-episode result of mutliAgent_ActionPolicy as a dict of [B] int32 device tensors, one per column of
+        gpp_outcome_field (include/gnnpp_b200.h); `valid` is 1 once an episode has ended and is scoreable."""
+        return {k: self.outcome_rows[:, i] for i, k in enumerate(_lib.OUTCOME_FIELDS)}
+
     # ------------------------------------------------------------------ the rollout loop (agents/...local.py:560-592)
     def run(self, model, max_steps: int = None, poll_every: int = 8):
         """Advances all episodes until every one has finished (all agents at their goals, or its maxstep reached).
         Per step: build_inputs -> model.addGSO + forward_logits -> move, all on the device; an episode stops being
-        moved once the reference's loop would have left it (:606-613).  Returns the number of steps taken."""
+        moved once the reference's loop would have left it (:606-613), and its outcome() is final from then on.
+        Returns the number of steps taken."""
         assert not model.training
         limit = int(self.maxstep.max().item()) if max_steps is None else int(max_steps)
         with torch.no_grad():
@@ -111,10 +146,10 @@ class BatchedRollout:
                 x, S = self.build_inputs(step)
                 model.addGSO(S)
                 logits = model.forward_logits(x)
-                flags = self.move(logits, step + 1)
+                self.move(logits, step + 1)
                 # the reference breaks after the move of the step at which all agents HAD reached their goals, or
-                # at maxstep: such episodes are frozen from the next step on
-                self.active = (self.active.bool() & ~flags[:, 0].bool() & (self.maxstep > step + 1)).to(torch.int32)
+                # at maxstep: record() writes such episodes' outcome and freezes them from the next step on
+                self.record(step + 1)
                 self.step = step + 1
                 if (step + 1) % poll_every == 0 and not bool(self.active.any().item()):
                     break

@@ -223,6 +223,63 @@ int gpp_rollout_move(const float* logits, int* pos, const int* goal, const unsig
                      int* last_action, unsigned int* choice_counter, int* flags, int currentstep, int B, int N,
                      int W, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Batched evaluation: the scoring half of agents/decentralplannerlocal.py:535-648 (mutliAgent_ActionPolicy) for B
+ * episodes advanced with gpp_rollout_move.  All pointers are device pointers, int32.
+ *
+ * gpp_rollout_expert_metrics replaces multiRobotSim.getPathTarget (utils/multirobotsim_dcenlocal.py:159-230); run once.
+ *   start, goal [B,N,2]; expert_action [B,N,T] action indices (0 up, 1 left, 2 down, 3 right, 4 stop).
+ *   Each agent replays its T actions from its start, ignoring obstacles and other agents.  startStep = first step
+ *   whose action is not stop; endStep = step + 1 at the first arrival on the goal.
+ *   makespan_target [B] = max(endStep) - min(startStep), flowtime_target [B] = sum(endStep - startStep), target_valid [B]
+ *   = 1 when both are usable as divisors: every agent arrives, every agent moves (the reference computes end - None
+ *   otherwise), all actions are in 0..4 and neither target is 0.  Unusable targets are written as 0, which is also
+ *   what the reference keeps when some agent never arrives.
+ *
+ * gpp_rollout_record: the per-step bookkeeping of mutliAgent_ActionPolicy (:555-624); call it after every
+ * gpp_rollout_move with the same active, flags and currentstep.  Episodes with active[b] == 0 are skipped (their flags
+ * are stale).  For the others the collision flags are OR-ed into the record; the episode ends when flags[b][0] (all
+ * agents had reached their goals before the move) is set or currentstep >= maxstep[b].  Then the whole row of
+ * outcome[b] is written and active[b] is cleared.
+ *   outcome [B, GPP_OUTCOME_FIELDS]: zero it before the first step.
+ *   makespan_target / flowtime_target: [B] from gpp_rollout_expert_metrics, or makespan_target == NULL when no expert
+ *   is given (the target columns and GPP_OUTCOME_FIND_OPTIMAL are then 0).
+ * The columns follow the reference, quirks included:
+ *   MAKESPAN_PREDICT / FLOWTIME_PREDICT = max(end) - min(start) / sum(end - start) of the last move only when
+ *     checkOptimality ran (collision-free success, or currentstep >= maxstep); otherwise the pre-loop defaults
+ *     maxstep / maxstep * N of getOptimalityMetrics (:555).
+ *   FIND_OPTIMAL = collision-free success with predicted <= target on both, reset to 0 when currentstep >= maxstep.
+ *   ALL_REACH_GOAL is flags[b][0] of the last move: agents that arrive on the maxstep move do not count.
+ *   NO_REACH_GOAL_SH = timeout and not ALL_REACH_GOAL and COLLISION_PREDICTED and not COLLISION_HAPPENED.
+ *   COLLISION_FREE = ALL_REACH_GOAL and not COLLISION_HAPPENED.   STEPS = the final currentStep.
+ *   VALID = 1 once the episode has ended and the reference would score it without raising: every predicted start step
+ *     is defined and (with targets) both targets are nonzero.
+ * ---------------------------------------------------------------------------------- */
+typedef enum gpp_outcome_field {
+    GPP_OUTCOME_STEPS = 0,
+    GPP_OUTCOME_ALL_REACH_GOAL = 1,
+    GPP_OUTCOME_NO_REACH_GOAL_SH = 2,
+    GPP_OUTCOME_FIND_OPTIMAL = 3,
+    GPP_OUTCOME_COLLISION_FREE = 4,
+    GPP_OUTCOME_COLLISION_PREDICTED = 5,
+    GPP_OUTCOME_COLLISION_HAPPENED = 6,
+    GPP_OUTCOME_NUM_REACH_GOAL = 7,
+    GPP_OUTCOME_MAKESPAN_PREDICT = 8,
+    GPP_OUTCOME_MAKESPAN_TARGET = 9,
+    GPP_OUTCOME_FLOWTIME_PREDICT = 10,
+    GPP_OUTCOME_FLOWTIME_TARGET = 11,
+    GPP_OUTCOME_VALID = 12,
+    GPP_OUTCOME_FIELDS = 13
+} gpp_outcome_field;
+
+/* replaces multiRobotSim.getPathTarget (utils/multirobotsim_dcenlocal.py:159-230) */
+int gpp_rollout_expert_metrics(const int* start, const int* goal, const int* expert_action, int T,
+                               int* makespan_target, int* flowtime_target, int* target_valid, int B, int N, void* stream);
+/* per-step outcome bookkeeping of mutliAgent_ActionPolicy (agents/decentralplannerlocal.py:555-624) */
+int gpp_rollout_record(const int* flags, const int* maxstep, const int* reached, const int* start_step,
+                       const int* end_step, const int* makespan_target, const int* flowtime_target,
+                       int* active, int* outcome, int currentstep, int B, int N, void* stream);
+
 /* Asynchronous variant for pipelined rollouts over INDEPENDENT episode batches: stages the inputs on a copy stream,
  * enqueues the forward on one of the planner's four compute streams (tickets rotate over them, so the feature kernel of
  * one batch runs next to the kernels of the batches before it on the SMs they leave idle) and returns at once with a completion ticket; the
