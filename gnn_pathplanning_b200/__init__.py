@@ -14,9 +14,10 @@ from .graphml import (BatchLSIGF, GraphFilterBatch, GraphFilterL2ShareBatch, Gra
                       graph_filter, torchpermul, FEATURE_MAJOR, NODE_MAJOR)
 from .planner import DecentralPlannerNet, planner_loss, weights_init
 from .rollout import BatchedRollout
-from .metrics import RolloutMetrics, evaluate
+from .metrics import RolloutMetrics, collect_failure_cases, evaluate
+from .expert_data import ExpertDataset, ExpertSolutions, FailureCases, load_expert_solutions
 
-__all__ = ["DecentralPlannerNet", "GraphFilterBatch", "BatchLSIGF", "graph_filter", "weights_init", "planner_loss", "BatchedRollout", "evaluate", "RolloutMetrics", "GraphFilterRNNBatch", "GraphFilterMoRNNBatch", "GraphFilterL2ShareBatch", "torchpermul",
+__all__ = ["DecentralPlannerNet", "GraphFilterBatch", "BatchLSIGF", "graph_filter", "weights_init", "planner_loss", "BatchedRollout", "evaluate", "RolloutMetrics", "collect_failure_cases", "ExpertDataset", "ExpertSolutions", "FailureCases", "load_expert_solutions", "GraphFilterRNNBatch", "GraphFilterMoRNNBatch", "GraphFilterL2ShareBatch", "torchpermul",
            "FEATURE_MAJOR", "NODE_MAJOR", "install_dropin", "build"]
 
 

@@ -80,12 +80,8 @@ def _stack_cases(loader, num_agents, rate_maxstep):
     return np.stack(starts), np.stack(goals), np.stack(maps), act, np.array(maxsteps, np.int32)
 
 
-def evaluate(model, loader, config, poll_every: int = 8) -> RolloutMetrics:
-    """Scores `model` on every case of `loader` the way the reference's `agent.test(mode)` does, in one batched,
-    device-resident run.  `loader` yields what the reference's test loader yields (the loader itself works); all cases
-    must share the number of agents and the map size.  `config` supplies num_agents, rate_maxstep, commR and device,
-    as in the reference.  Raises ValueError naming the cases the reference's test() would fail on (an expert path that
-    leaves some agent short of its goal, an agent whose expert or predicted path never records a start step)."""
+def _run_test_set(model, loader, config, poll_every):
+    """The batched rollout of `evaluate`: returns (rollout, outcome columns, maxstep [B], goal [B,N,2], maps [B,W,W])."""
     N = int(config.num_agents)
     rate = 3 if N >= 20 else int(config.rate_maxstep)               # multirobotsim_dcenlocal.py:76-79
     start, goal, maps, act, maxstep = _stack_cases(loader, N, rate)
@@ -103,4 +99,26 @@ def evaluate(model, loader, config, poll_every: int = 8) -> RolloutMetrics:
     if bad.size:
         raise ValueError("evaluate: the reference's test() cannot score cases %s: an expert path that does not reach "
                          "every goal, or an agent that reaches its goal without ever moving" % bad.tolist())
-    return RolloutMetrics(outcome)
+    return ro, outcome, maxstep, goal, maps
+
+
+def evaluate(model, loader, config, poll_every: int = 8) -> RolloutMetrics:
+    """Scores `model` on every case of `loader` the way the reference's `agent.test(mode)` does, in one batched,
+    device-resident run.  `loader` yields what the reference's test loader yields (the loader itself works); all cases
+    must share the number of agents and the map size.  `config` supplies num_agents, rate_maxstep, commR and device,
+    as in the reference.  Raises ValueError naming the cases the reference's test() would fail on (an expert path that
+    leaves some agent short of its goal, an agent whose expert or predicted path never records a start step)."""
+    return RolloutMetrics(_run_test_set(model, loader, config, poll_every)[1])
+
+
+def collect_failure_cases(model, loader, config, poll_every: int = 8):
+    """`evaluate` plus the online expert's failure cases: the reference's test('test_trainingSet') with
+    switch_toOnlineExpert (agents/decentralplannerlocal_OnlineExpert.py:536-539) saves every case whose loop ended
+    with currentStep >= maxstep, whether or not all agents had arrived, starting each agent from its cell after the
+    last move.  Returns (RolloutMetrics, FailureCases); the start cells are gathered from the frozen rollout on the
+    device.  Same arguments and errors as `evaluate`."""
+    from .expert_data import FailureCases
+    ro, outcome, maxstep, goal, maps = _run_test_set(model, loader, config, poll_every)
+    idx = np.nonzero(outcome["steps"] >= maxstep)[0]
+    start = ro.pos.index_select(0, torch.from_numpy(idx).to(ro.pos.device))
+    return RolloutMetrics(outcome), FailureCases(idx, start, goal[idx], maps[idx])

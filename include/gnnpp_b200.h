@@ -280,6 +280,38 @@ int gpp_rollout_record(const int* flags, const int* maxstep, const int* reached,
                        const int* end_step, const int* makespan_target, const int* flowtime_target,
                        int* active, int* outcome, int currentstep, int B, int N, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Device-resident expert dataset: the training samples the reference's online-expert DataTransformer writes as one
+ * .mat file per case (onlineExpert/DataTransformer_local_onlineExpert.py:154-305) and its loader slices into one sample
+ * per step (dataloader/Dataloader_dcplocal_notTF_onlineExpert.py:142-157), built on demand from integer states.
+ * All pointers are device pointers.  The cases share N (2 <= N <= 64, else GPP_ERR_UNSUPPORTED) and the map size W.
+ *   states       [R,N,2] int32: the T = makespan + 1 states of every case, case after case (agent i at step t is at
+ *                its path's cell t while t < len(path), at its goal after that)
+ *   case_offset  [C] int32: row of each case's step 0;  case_steps [C] int32: its T
+ *   goal         [C,N,2] int32
+ *
+ * gpp_expert_radius replaces computeAdjacencyMatrix (:256-305) and the move check of obtainSchedule (:177-189); run
+ * once per case.  radius [C] f64 out: init_radius (the transformer's constant 5) multiplied by 1.1 at every step, in
+ * order, that is not connected under the current value (the value carries over to the next step).  valid [C] int32
+ * out: 1 when every move state[t] -> state[t+1] (the goal after the last state) is one of the five deltas; bad [C,2]
+ * int32 out: (step, agent) of the first other move in the reference's order (agent after agent), else (-1, -1).
+ *
+ * gpp_expert_gather: B samples, sample = state row (step t of case c is row case_offset[c] + t).
+ *   row_case [R] int32: case of every row;  map [C,W,W] uint8, 1 = obstacle;  radius [C] from gpp_expert_radius
+ *   rows [B] int64: the samples; a row outside 0..R-1 leaves its outputs unwritten
+ *   x             out f32 [B,N,3,11,11] or NULL: AgentState.toSeqInputTensor at the sample's state
+ *   target_onehot out int64 [B,N,5] or NULL: the one-hot action state[t] -> state[t+1] (the goal after the last state)
+ *   S             out [B,N,N] f64 (s_is_f64) or f32, or NULL: D^-1/2 A D^-1/2, A = (pdist < radius[c]) with a zero
+ *                 diagonal, computed in float64 (f32 = rounded, as the loader's .float())
+ * Bit-exact with the reference for the cases gpp_expert_radius marks valid.
+ * ---------------------------------------------------------------------------------- */
+int gpp_expert_radius(const int* states, const int* case_offset, const int* case_steps, const int* goal,
+                      double init_radius, double* radius, int* valid, int* bad, int C, int N, void* stream);
+int gpp_expert_gather(const int* states, const int* case_offset, const int* case_steps, const int* row_case,
+                      const int* goal, const unsigned char* map, const double* radius, const long long* rows,
+                      float* x, long long* target_onehot, void* S, int s_is_f64, int B, int N, int W, int R,
+                      void* stream);
+
 /* Asynchronous variant for pipelined rollouts over INDEPENDENT episode batches: stages the inputs on a copy stream,
  * enqueues the forward on one of the planner's four compute streams (tickets rotate over them, so the feature kernel of
  * one batch runs next to the kernels of the batches before it on the SMs they leave idle) and returns at once with a completion ticket; the
