@@ -312,6 +312,59 @@ int gpp_expert_gather(const int* states, const int* case_offset, const int* case
                       float* x, long long* target_onehot, void* S, int s_is_f64, int B, int N, int W, int R,
                       void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Batched expert solver (replaces the reference's prebuilt `ecbs -w 1.1` binary, run by onlineExpert/ECBS_onlineExpert.py
+ * on the online expert's failure cases and by offlineExpert/CasesGenerator.py:283-340 on the offline dataset).
+ * Conflict-based search (CBS) minimising the sum of costs (SoC): the SoC it returns is optimal among the solutions with
+ * makespan <= H, which meets ECBS's guarantee (SoC <= w x optimal).  One warp per case, C cases per call.
+ *
+ * Move model (the reference simulator's): the five actions up (-1,0), left (0,-1), down (1,0), right (0,1), stop;
+ * obstacles and the map edge are blocked; two agents on one cell at one step (vertex conflict) and two agents trading
+ * cells in one step (swap conflict) are forbidden; an agent stays on its goal after its path ends.  Agent i's cost tau_i
+ * is the step after which it stays on its goal; the case's makespan is max tau_i.
+ *
+ * Every tie is fixed, so the solution is a function of the input:
+ *   low level (agent i under its constraints): L_0 = {start}; L_{t+1} = the free cells v not vertex-constrained at t+1
+ *     with some u in L_t, v in {u, u + delta}, (u -> v, t) not edge-constrained.  tau_i = the smallest t <= H with
+ *     goal in L_t and t > the latest vertex constraint on the goal (or -1); none: the node is infeasible.  The path is
+ *     backtracked from (goal, tau_i): at each step the first predecessor p in L_{t-1} whose move p -> c is not
+ *     edge-constrained, trying the actions in the order stop, up, left, down, right (p = c - delta).
+ *   conflict: the earliest t; at that t vertex conflicts (pairs i < j, lexicographic) before swap conflicts between t
+ *     and t+1 (i < j, lexicographic); paths are extended with their goal.
+ *   high level: expand the open node with the smallest (SoC, creation index); the root has index 0.  The child that
+ *     constrains i is created before the one that constrains j: a vertex conflict at (v, t) adds the vertex constraint
+ *     (v, t); a swap with i moving u -> v adds (u -> v, t) for i and (v -> u, t) for j.  Only the constrained agent is
+ *     replanned; an infeasible child is not created and takes no index.
+ *   stop: GPP_SOLVE_SOLVED when the expanded node has no conflict; GPP_SOLVE_NO_SOLUTION when an agent of the root is
+ *     infeasible or the open list runs empty (no solution has makespan <= H); GPP_SOLVE_BUDGET when a feasible child
+ *     would be node number max_nodes + 1.
+ *
+ * All pointers are device pointers.  Envelope: 1 <= N <= 64, 1 <= W <= 64, 1 <= H <= 1024, 1 <= max_nodes <= 65536,
+ * else GPP_ERR_UNSUPPORTED.  The caller guarantees distinct starts, distinct goals and free in-map cells.
+ *   map [C,W,W] uint8 (nonzero = obstacle);  start, goal [C,N,2] int32 cells (x, y)
+ *   status [C] (gpp_solve_status);  soc, makespan [C] (-1 unless solved)
+ *   nodes_created, nodes_expanded [C] (the root counts as created, the solved node as expanded)
+ *   low_level [C]: single-agent searches run (the root's, stopping at the first infeasible agent, and one per child)
+ *   tau [C,N] (-1 unless solved);  paths [C,N,H+1] int16: agent i's cell x * W + y at every step, the goal after
+ *   tau_i (-1 unless solved)
+ *   workspace: gpp_expert_solve_workspace_bytes(C, N, W, H, max_nodes) bytes of device scratch.  It is sized per
+ *   resident warp, not per case: 256 + warps * per-warp bytes, warps = min(C, resident warps, 2 GiB / per-warp bytes),
+ *   per-warp bytes = 8 W (H+1) layers + 56 max_nodes (nodes, open list, constraints) + 2 (N + max_nodes)(H+1) paths,
+ *   each part rounded up to 256 bytes.
+ * ---------------------------------------------------------------------------------- */
+typedef enum gpp_solve_status {
+    GPP_SOLVE_SOLVED = 0,
+    GPP_SOLVE_NO_SOLUTION = 1,
+    GPP_SOLVE_BUDGET = 2
+} gpp_solve_status;
+
+/* 0 outside the envelope or for C <= 0 */
+size_t gpp_expert_solve_workspace_bytes(int C, int N, int W, int H, int max_nodes);
+int gpp_expert_solve(const unsigned char* map, const int* start, const int* goal, int H, int max_nodes,
+                     int* status, int* soc, int* makespan, int* nodes_created, int* nodes_expanded, int* low_level,
+                     int* tau, short* paths, void* workspace, size_t workspace_bytes, int C, int N, int W,
+                     void* stream);
+
 /* Asynchronous variant for pipelined rollouts over INDEPENDENT episode batches: stages the inputs on a copy stream,
  * enqueues the forward on one of the planner's four compute streams (tickets rotate over them, so the feature kernel of
  * one batch runs next to the kernels of the batches before it on the SMs they leave idle) and returns at once with a completion ticket; the
