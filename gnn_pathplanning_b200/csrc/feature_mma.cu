@@ -21,14 +21,17 @@
 //   linear 1 x 1              8      16      128     1        1 x 8        64 KB
 //
 // Precision: v = hi + lo with hi = fp16(v * 2^e), lo = fp16(v * 2^e - hi); products hi*hi + lo*hi + hi*lo accumulate
-// in one fp32 register accumulator.  e is chosen per agent and layer from the running maximum (two-pass epilogue),
-// weights are scaled per layer; residual ~2^-22 per product.  For N <= 64 the filter image holds [W_hi | W_lo] side
-// by side (2N rows per K plane); for N = 128 the two are separate 128-row planes.
+// in fp32 registers.  e is chosen per agent and layer from the running maximum (two-pass epilogue),
+// weights are scaled per layer; residual ~2^-22 per product.  Each K plane of a filter image holds, per warpgroup's
+// channel group, [W_hi | W_lo] rows side by side, so A_hi x (W_hi, W_lo) is ONE MMA of twice the width and A_lo x W_hi
+// a second; the hi.lo half of the accumulator is added to the rest after the layer.
 //
-// Roles: warps 0-7 = two warpgroups, one per half of the output channels: each issues the wgmma of its channels for
-// all rows (M = 64 per instruction), stages its accumulators through shared memory and runs the epilogue
-// (BatchNorm/ReLU/max-pool -> fp16 split -> next layer's operand buffer); warp 8 = loader (filter chunks through a
-// 5 x 16 KB ring of bulk copies, input tiles).
+// Roles: warps 0-7 = two warpgroups.  conv0..conv2 (several 64-row blocks) split the rows: warpgroup h computes block h
+// of every 128-row M tile for all output channels; conv3, conv4 and the linear layer (one block) split the channels.
+// Each warpgroup issues its wgmma (M = 64 per instruction; a chunk's ring slot is released one chunk later, so the
+// MMAs stream), stages its accumulators through shared memory and runs the epilogue (BatchNorm/ReLU/max-pool -> fp16
+// split -> next layer's operand buffer); warps 8-11 = loader warpgroup, one lane of which streams filter chunks
+// through a 5 x 16 KB ring of bulk copies and the input tiles; it gives its registers to the compute warpgroups.
 #include "common.cuh"
 #include "feature.cuh"
 #include "tc_common.cuh"
@@ -42,7 +45,8 @@ constexpr int FM_A = 8;                        // agents per tile
 constexpr int FM_EPI_WARPS = 8;
 constexpr int FM_EPI_THREADS = 32 * FM_EPI_WARPS;
 constexpr int FM_LOADER_WARP = FM_EPI_WARPS;
-constexpr int FM_THREADS = FM_EPI_THREADS + 32;
+constexpr int FM_THREADS = FM_EPI_THREADS + 128;   // + a loader warpgroup, of which one lane works (setmaxnreg)
+constexpr int FM_LOADER_REGS = 40, FM_EPI_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
 constexpr int FM_SLOTS = 5, FM_SLOT_BYTES = 16384;
 constexpr int FM_NL = 6;
 
@@ -62,6 +66,14 @@ __host__ __device__ constexpr int fm_unit_bytes(int L) { return L == 0 ? 6144 : 
 __host__ __device__ constexpr int fm_upc(int L) { return L == 0 ? 1 : L == 1 ? 8 : L < 4 ? 4 : 2; }   // units per chunk
 __host__ __device__ constexpr int fm_chunks(int L) { return (fm_units(L) + fm_upc(L) - 1) / fm_upc(L); }
 __host__ __device__ constexpr int fm_img_bytes(int L) { return fm_units(L) * fm_unit_bytes(L); }
+// Work split between the two warpgroups.  conv0..conv2 have several 64-row blocks per 128-row M tile: warpgroup h takes
+// block h of every M tile for ALL output channels, so each A row is read by one warpgroup only.  conv3, conv4 and the
+// linear layer have one block: warpgroup h takes half h of the output channels.
+__host__ __device__ constexpr bool fm_rowsplit(int L) { return L <= 2; }
+__host__ __device__ constexpr int fm_nc(int L) { return fm_rowsplit(L) ? fm_n(L) : fm_n(L) / 2; }     // channels per WG
+// Layers 1..5 issue A_hi x [W_hi | W_lo] as one MMA of width 2 NC (the W_lo half of the accumulator is added to the
+// W_hi half after the layer), then A_lo x W_hi: two instructions per product instead of three.
+__host__ __device__ constexpr int fm_af(int L) { return fm_nc(L); }     // accumulator floats per 64-row block
 
 // shared-memory map (bytes from the 1024-aligned base)
 constexpr int FM_R1 = 0;                           // in0 (hi|lo) -> act2 -> act4
@@ -176,21 +188,22 @@ struct FmRing {
 };
 __device__ __forceinline__ uint64_t fm_desc(uint32_t addr, uint32_t lbo) { return gmma_desc_nosw(addr, lbo, 128); }
 
-// ---- MMAs of one layer L >= 1 for this warpgroup's half h of the output channels: acc[t][mh] = rows t * 128 + 64 mh ..
-//      of the layer's M tiles, N / 2 channels.  Every descriptor offset is a compile-time constant (fully unrolled).
+// ---- MMAs of one layer L >= 1 for warpgroup h: acc[t] = rows t * 128 + (row split ? 64 h : 0) .. + 63 of the layer's
+//      M tiles, fm_nc(L) channels (after the layer, the first fm_nc(L) / 2 floats).  Every descriptor offset but the
+//      warpgroup's own is a compile-time constant (fully unrolled).  A chunk's ring slot is freed once the MMAs of the
+//      NEXT chunk are issued (wait_group 1), so the tensor pipe does not drain at every chunk.
 template <int L>
-__device__ __forceinline__ constexpr int fm_mh() { return L >= 3 ? 1 : 2; }     // conv3 / conv4 / linear: rows < 64 only
-
-template <int L, typename Acc>
-__device__ __forceinline__ void fm_mma_layer(uint32_t sm_base, FmMisc* ms, FmRing& ring, int h, Acc& acc, unsigned long long* tacc) {
-    constexpr int N = fm_n(L), NW = N / 2, KS = fm_ks(L), UNITS = fm_units(L), UPC = fm_upc(L), UB = fm_unit_bytes(L);
-    constexpr int AW = fm_aw(L), LBO = (L == 5) ? 128 : fm_lbo(L), TILES = fm_tiles(L), MH = fm_mh<L>();
+__device__ __forceinline__ void fm_mma_layer(uint32_t sm_base, FmMisc* ms, FmRing& ring, int h, float (&acc)[fm_tiles(L)][fm_af(L)],
+                                             unsigned long long* tacc) {
+    constexpr int NC = fm_nc(L), KS = fm_ks(L), UNITS = fm_units(L), UPC = fm_upc(L), UB = fm_unit_bytes(L);
+    constexpr int AW = fm_aw(L), LBO = (L == 5) ? 128 : fm_lbo(L), TILES = fm_tiles(L);
     constexpr uint32_t A_HI = fm_in_base(L), A_LO = fm_in_base(L) + fm_planes(L) * LBO;
     constexpr int CHUNKS = fm_chunks(L);
-    // B rows of this channel half: [W_hi | W_lo] planes of 2N rows (N <= 64), or separate 128-row W_hi / W_lo planes
-    const uint32_t b_hi_off = (L <= 3) ? (uint32_t)(h * NW * 16) : (uint32_t)(h * 64 * 16);
-    const uint32_t b_lo_off = (L <= 3) ? (uint32_t)((N + h * NW) * 16) : (uint32_t)(4096 + h * 64 * 16);
-    constexpr uint32_t BLBO = (L <= 3) ? 32 * N : 2048;
+    // B planes of 2N rows; this warpgroup's NC channels are [W_hi NC rows | W_lo NC rows] in them (fm_prep_image_kernel)
+    constexpr uint32_t BLBO = 32 * fm_n(L);
+    const uint32_t b_off = fm_rowsplit(L) ? 0u : (uint32_t)(h * 2 * NC * 16);
+    const uint32_t a_off = fm_rowsplit(L) ? (uint32_t)(h * 64 * 16) : 0u;
+    uint32_t prev = 0;
 #pragma unroll
     for (int cc = 0; cc < CHUNKS; ++cc) {
         {
@@ -199,7 +212,8 @@ __device__ __forceinline__ void fm_mma_layer(uint32_t sm_base, FmMisc* ms, FmRin
             FM_ACC(6 + L);
         }
         FM_T0();
-        const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES;
+        const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES + b_off;
+        const uint32_t as = sm_base + a_off;
         wgmma_fence();
 #pragma unroll
         for (int uu = 0; uu < UPC; ++uu) {
@@ -207,24 +221,34 @@ __device__ __forceinline__ void fm_mma_layer(uint32_t sm_base, FmMisc* ms, FmRin
             if (u < UNITS) {
                 const int tap = u / KS, k16 = u - tap * KS;
                 const int shift = (L == 5) ? 0 : ((tap / 3) * AW + (tap % 3));
-                const uint64_t db_hi = fm_desc(bs + uu * UB + b_hi_off, BLBO), db_lo = fm_desc(bs + uu * UB + b_lo_off, BLBO);
+                const uint64_t db = fm_desc(bs + uu * UB, BLBO);
 #pragma unroll
-                for (int t = 0; t < TILES; ++t)
-#pragma unroll
-                    for (int mh = 0; mh < MH; ++mh) {
-                        const uint32_t aoff = (uint32_t)((t * 128 + mh * 64 + shift) * 16 + k16 * 2 * LBO);
-                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_HI + aoff, LBO), db_hi, u > 0);
-                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_LO + aoff, LBO), db_hi, 1);
-                        wgmma_f16<NW>(acc[t][mh], fm_desc(sm_base + A_HI + aoff, LBO), db_lo, 1);
-                    }
+                for (int t = 0; t < TILES; ++t) {
+                    const uint32_t aoff = (uint32_t)((t * 128 + shift) * 16 + k16 * 2 * LBO);
+                    wgmma_f16<2 * NC>(acc[t], fm_desc(as + A_HI + aoff, LBO), db, u > 0);
+                    wgmma_f16<NC>(acc[t], fm_desc(as + A_LO + aoff, LBO), db, 1);
+                }
             }
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        fm_arrive_warp(&ms->w_free[ring.slot]);
+        if (cc > 0) {
+            wgmma_wait<1>();
+            fm_arrive_warp(&ms->w_free[prev]);
+        }
+        prev = ring.slot;
         ring.advance();
         FM_ACC(12 + L);
     }
+    {
+        FM_T0();
+        wgmma_wait<0>();
+        fm_arrive_warp(&ms->w_free[prev]);
+        FM_ACC(12 + L);
+    }
+#pragma unroll
+    for (int t = 0; t < TILES; ++t)
+#pragma unroll
+        for (int i = 0; i < NC / 2; ++i) acc[t][i] += acc[t][i + NC / 2];
 }
 
 // ---- epilogue pieces -----------------------------------------------------------------------------------------------
@@ -286,7 +310,7 @@ __host__ __device__ constexpr int fm_srow(int L) { return fm_n(L) + 4; }
 template <int L>
 __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_base, FmMisc* ms, FmRing& ring, int na,
                                                 int q, int h, int lane, int et, unsigned long long* tacc) {
-    constexpr int N = fm_n(L), AW = fm_aw(L), WP = fm_wp(L), HO = fm_hout(L), TILES = fm_tiles(L), MH = fm_mh<L>();
+    constexpr int N = fm_n(L), AW = fm_aw(L), WP = fm_wp(L), HO = fm_hout(L), TILES = fm_tiles(L);
     constexpr bool POOL = (L == 2 || L == 4);
     constexpr int LO = L + 1;                                      // the layer that consumes the output
     constexpr uint32_t OUT = fm_in_base(LO);
@@ -295,7 +319,7 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
     constexpr int CV = POOL ? 8 : 16;
     constexpr int SROW = fm_srow(L);
     const int wt = et & 127;                                       // thread of the warpgroup
-    float acc[TILES][MH][N / 4];
+    float acc[TILES][fm_af(L)];
     fm_mma_layer<L>(sm_base, ms, ring, h, acc, tacc);
     fm_epi_sync();                                                 // both warpgroups' MMAs are done with the input buffer
     FM_T0();
@@ -311,12 +335,11 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
     for (int t = 0; t < TILES; ++t) {
         if (t > 0) fm_epi_sync();                                   // pass 1 of tile t - 1 has read the staging buffer
 #pragma unroll
-        for (int mh = 0; mh < MH; ++mh)
-#pragma unroll
-            for (int i = 0; i < N / 4; i += 2) {
-                const int row = 64 * mh + wg_row(wt, i), col = h * (N / 2) + wg_col(wt, i);
-                *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[t][mh][i], acc[t][mh][i + 1]);
-            }
+        for (int i = 0; i < fm_nc(L) / 2; i += 2) {
+            const int row = (fm_rowsplit(L) ? 64 * h : 0) + wg_row(wt, i);
+            const int col = (fm_rowsplit(L) ? 0 : h * (N / 2)) + wg_col(wt, i);
+            *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[t][i], acc[t][i + 1]);
+        }
         fm_epi_sync();
         if (rows_here) {
             const int r = t * 128 + l;
@@ -388,6 +411,28 @@ __device__ __forceinline__ void fm_epilogue_dyn(unsigned char* sm, uint32_t sm_b
     FM_ACC(26 + L);
 }
 
+// conv0 MMAs of image rows 2j, 2j + 1 (acc[tt]) for the 64-row block that starts at a_hi, all 32 channels; LO: the
+// inputs are not fp16-exact, add their lo planes.  The choice is made outside the instruction sequence: a branch
+// between two wgmma makes the compiler serialise them.
+template <bool LO>
+__device__ __forceinline__ void fm_conv0_mma(float (&acc)[2][16], uint32_t a_hi, uint32_t bs, int j) {
+    wgmma_fence();
+#pragma unroll
+    for (int tt = 0; tt < 2; ++tt) {
+        const uint32_t arow = (uint32_t)((2 * j + tt) * 128);      // rows of 16 bytes
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+            for (int pr = 0; pr < 2; ++pr) {        // K = 16 = image rows ky = 2 pr, 2 pr + 1 (LBO = one row)
+                const uint32_t aoff = (arow + 2 * pr * 128 + kx) * 16;
+                const uint64_t db = fm_desc(bs + (kx * 2 + pr) * 1024, 512);
+                wgmma_f16<32>(acc[tt], fm_desc(a_hi + aoff, 2048), db, (kx | pr) != 0);
+                if constexpr (LO) wgmma_f16<32>(acc[tt], fm_desc(a_hi + fm_lbo(0) + aoff, 2048), db, 1);
+            }
+    }
+    wgmma_commit();
+}
+
 // =====================================================================================================================
 __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs A) {
     extern __shared__ __align__(1024) unsigned char sm[];
@@ -405,9 +450,12 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
     unsigned long long* tacc = (blockIdx.x == 0 && threadIdx.x == 0) ? A.timing : nullptr;
     griddep_launch_dependents();       // the next kernel of the stream may start its prologue; it still waits for this grid
 
-    if (warp == FM_LOADER_WARP) {
+    if (warp >= FM_LOADER_WARP) {
         // ================= loader =================
-        if (lane == 0) {
+        // Its warpgroup hands its registers to the compute warpgroups: with a lone 9th warp instead, 3 warps share one
+        // SM sub-partition and every thread is capped at 168 registers, which made the epilogues spill.
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(FM_LOADER_REGS));
+        if (warp == FM_LOADER_WARP && lane == 0) {
             uint32_t g = 0;
             int it = 0;
             auto issue_x = [&](int tile) {
@@ -447,7 +495,8 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
             }
         }
     } else {
-        // ================= compute warps: two warpgroups = channel halves h =================
+        // ================= compute warps: two warpgroups (fm_rowsplit: row blocks or channel halves h) =================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(FM_EPI_REGS));
         const int q = warp & 3, h = warp >> 2, et = threadIdx.x, wt = et & 127;
         FmRing ring;
         ring.slot = 0; ring.phase = 0;
@@ -519,62 +568,45 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
             fm_epi_sync();                     // xflag / act1 zeroes / in0 complete in every warp
             if (tacc) atomicAdd(&tacc[19], (unsigned long long)(clock64() - t_conv0));
 
-            // ---- conv0: five pairs of image rows (M tiles 2j, 2j + 1 = image rows y = 2j, 2j + 1 of the 8 agents), this
-            //      warpgroup's 16 channels; y pairs are the two accumulators, x pairs rows l ^ 1 = lanes 4 apart
+            // ---- conv0: five pairs of image rows (M tiles 2j, 2j + 1 = image rows y = 2j, 2j + 1 of the 8 agents); this
+            //      warpgroup's 64-row block = agents 4h .. 4h + 3, all 32 channels; y pairs are the two accumulators, x
+            //      pairs rows l ^ 1 = lanes 4 apart
             {
                 const bool has_lo = ms->xflag != 0;
                 FM_T0();
                 fm_wait(&ms->w_full[ring.slot], ring.phase);
                 FM_ACC(6);
-                const uint32_t a_hi = sm_base + FM_R1, a_lo = a_hi + fm_lbo(0);
-                const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES + h * 16 * 16;
-                const int c0 = h * 16;
+                const uint32_t a_hi = sm_base + FM_R1 + h * 64 * 16;
+                const uint32_t bs = sm_base + FM_RING + ring.slot * FM_SLOT_BYTES;
                 const float* cs = reinterpret_cast<const float*>(sm + FM_CST);
                 for (int j = 0; j < 5; ++j) {
-                    float acc[2][2][8];           // [tt][mh]
-                    wgmma_fence();
-#pragma unroll
-                    for (int tt = 0; tt < 2; ++tt)
-#pragma unroll
-                        for (int mh = 0; mh < 2; ++mh) {
-                            const uint32_t arow = (uint32_t)((2 * j + tt) * 128 + 64 * mh);      // rows of 16 bytes
-#pragma unroll
-                            for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-                                for (int pr = 0; pr < 2; ++pr) {        // K = 16 = image rows ky = 2 pr, 2 pr + 1 (LBO = one row)
-                                    const uint32_t aoff = (arow + 2 * pr * 128 + kx) * 16;
-                                    const uint64_t db = fm_desc(bs + (kx * 2 + pr) * 1024, 512);
-                                    wgmma_f16<16>(acc[tt][mh], fm_desc(a_hi + aoff, 2048), db, (kx | pr) != 0);
-                                    if (has_lo) wgmma_f16<16>(acc[tt][mh], fm_desc(a_lo + aoff, 2048), db, 1);
-                                }
-                        }
-                    wgmma_commit();
+                    float acc[2][16];           // [tt]
+                    if (has_lo) fm_conv0_mma<true>(acc, a_hi, bs, j);
+                    else fm_conv0_mma<false>(acc, a_hi, bs, j);
                     wgmma_wait<0>();
 #pragma unroll
-                    for (int mh = 0; mh < 2; ++mh)
+                    for (int i = 0; i < 16; i += 2) {
+                        const int row = 64 * h + wg_row(wt, i), c = wg_col(wt, i);
+                        const int a = row >> 4, x = row & 15;
+                        const float inv = ms->inv0[a], mul = ms->mul1[a];
+                        float v[2];
 #pragma unroll
-                        for (int i = 0; i < 8; i += 2) {
-                            const int row = 64 * mh + wg_row(wt, i), c = c0 + wg_col(wt, i);
-                            const int a = row >> 4, x = row & 15;
-                            const float inv = ms->inv0[a], mul = ms->mul1[a];
-                            float v[2];
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const float k = cs[c + e] * inv, sh = cs[128 + c + e];
-                                const float u = fmaxf(fmaxf(fmaf(acc[0][mh][i + e], k, sh), fmaf(acc[1][mh][i + e], k, sh)), 0.f);
-                                v[e] = fmaxf(u, __shfl_xor_sync(0xffffffffu, u, 4)) * mul;
-                            }
-                            if ((x & 1) == 0 && x < 10 && a < na) {
-                                const int orow = fm_aw(1) + a * fm_wp(1) + (x >> 1) + 1 + j * fm_aw(1);
-                                const __half2 hh = __floats2half2_rn(v[0], v[1]);
-                                const float2 f = __half22float2(hh);
-                                const __half2 ll = __floats2half2_rn(v[0] - f.x, v[1] - f.y);
-                                const uint32_t addr = sm_base + FM_R2 + (c >> 3) * fm_lbo(1) + orow * 16 + (c & 7) * 2;
-                                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&hh)) : "memory");
-                                asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + fm_planes(1) * fm_lbo(1)),
-                                             "r"(*reinterpret_cast<const uint32_t*>(&ll)) : "memory");
-                            }
+                        for (int e = 0; e < 2; ++e) {
+                            const float k = cs[c + e] * inv, sh = cs[128 + c + e];
+                            const float u = fmaxf(fmaxf(fmaf(acc[0][i + e], k, sh), fmaf(acc[1][i + e], k, sh)), 0.f);
+                            v[e] = fmaxf(u, __shfl_xor_sync(0xffffffffu, u, 4)) * mul;
                         }
+                        if ((x & 1) == 0 && x < 10 && a < na) {
+                            const int orow = fm_aw(1) + a * fm_wp(1) + (x >> 1) + 1 + j * fm_aw(1);
+                            const __half2 hh = __floats2half2_rn(v[0], v[1]);
+                            const float2 f = __half22float2(hh);
+                            const __half2 ll = __floats2half2_rn(v[0] - f.x, v[1] - f.y);
+                            const uint32_t addr = sm_base + FM_R2 + (c >> 3) * fm_lbo(1) + orow * 16 + (c & 7) * 2;
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&hh)) : "memory");
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + fm_planes(1) * fm_lbo(1)),
+                                         "r"(*reinterpret_cast<const uint32_t*>(&ll)) : "memory");
+                        }
+                    }
                 }
                 fm_arrive_warp(&ms->w_free[ring.slot]);
                 ring.advance();
@@ -589,7 +621,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
             // ---- compress MLP: rows 0..7 of the tile are the agents
             {
                 constexpr int SROW = fm_srow(5);
-                float acc[1][1][32];
+                float acc[1][fm_af(5)];
                 fm_mma_layer<5>(sm_base, ms, ring, h, acc, tacc);
                 fm_epi_sync();
                 FM_T0();
@@ -597,7 +629,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) feature_mma_kernel(const FmArgs
 #pragma unroll
                 for (int i = 0; i < 32; i += 2) {
                     const int row = wg_row(wt, i), col = h * 64 + wg_col(wt, i);
-                    if (row < FM_A) *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[0][0][i], acc[0][0][i + 1]);
+                    if (row < FM_A) *reinterpret_cast<float2*>(sacc + row * SROW + col) = make_float2(acc[0][i], acc[0][i + 1]);
                 }
                 fm_epi_sync();
                 if (q == 0 && lane < FM_A && lane < na) {
@@ -656,24 +688,16 @@ __global__ void fm_prep_image_kernel(const float* __restrict__ w, __half* __rest
         const int ky = 2 * pr + p;
         islo = e >= 3;
         if (ky < 3 && e < 6) v = w[(n * 3 + (e % 3)) * 9 + ky * 3 + kx];
-    } else if (L <= 3) {
-        // [unit][plane][n2 (2N = hi | lo)][8]
-        const int Cin = fm_planes(L) * 8, KS = fm_ks(L);
-        int r = idx >> 3;
-        const int n2 = r % (2 * N); r /= 2 * N;
-        const int p = r & 1, u = r >> 1;
-        const int tap = u / KS, k16 = u - tap * KS, ci = k16 * 16 + p * 8 + e, n = n2 % N;
-        islo = n2 / N;
-        v = w[((size_t)n * Cin + ci) * 9 + tap];
     } else {
-        // [unit][hi | lo][plane][n (128)][8]
-        const int Cin = fm_planes(L) * 8, KS = fm_ks(L);
+        // [unit][plane][g][hi | lo][n (NC)][8]: one group g = the NC channels of a warpgroup (fm_nc), W_hi rows then W_lo
+        // rows, so that A_hi x [W_hi | W_lo] is one MMA of width 2 NC.  Row split layers: one group of all N channels.
+        const int Cin = fm_planes(L) * 8, KS = fm_ks(L), NC = fm_nc(L);
         int r = idx >> 3;
-        const int n = r & 127; r >>= 7;
-        const int p = r & 1; r >>= 1;
-        islo = r & 1;
-        const int u = r >> 1;
-        const int tap = u / KS, k16 = u - tap * KS, ci = k16 * 16 + p * 8 + e;
+        const int nl = r % NC; r /= NC;
+        islo = r & 1; r >>= 1;
+        const int G = N / NC, g = r % G; r /= G;
+        const int p = r & 1, u = r >> 1;
+        const int tap = u / KS, k16 = u - tap * KS, ci = k16 * 16 + p * 8 + e, n = g * NC + nl;
         v = (L == 5) ? w[(size_t)n * 128 + ci] : w[((size_t)n * Cin + ci) * 9 + tap];
     }
     img[idx] = fm_pick(v * mul, islo);
