@@ -17,8 +17,9 @@ from .rollout import BatchedRollout
 from .metrics import RolloutMetrics, collect_failure_cases, evaluate
 from .expert_data import ExpertDataset, ExpertSolutions, FailureCases, load_expert_solutions
 from .expert_solver import SolveResult, solve_cases
+from .case_gen import GeneratedCases, generate_cases
 
-__all__ = ["DecentralPlannerNet", "GraphFilterBatch", "BatchLSIGF", "graph_filter", "weights_init", "planner_loss", "BatchedRollout", "evaluate", "RolloutMetrics", "collect_failure_cases", "ExpertDataset", "ExpertSolutions", "FailureCases", "load_expert_solutions", "solve_cases", "SolveResult", "GraphFilterRNNBatch", "GraphFilterMoRNNBatch", "GraphFilterL2ShareBatch", "torchpermul",
+__all__ = ["DecentralPlannerNet", "GraphFilterBatch", "BatchLSIGF", "graph_filter", "weights_init", "planner_loss", "BatchedRollout", "evaluate", "RolloutMetrics", "collect_failure_cases", "ExpertDataset", "ExpertSolutions", "FailureCases", "load_expert_solutions", "solve_cases", "SolveResult", "generate_cases", "GeneratedCases", "GraphFilterRNNBatch", "GraphFilterMoRNNBatch", "GraphFilterL2ShareBatch", "torchpermul",
            "FEATURE_MAJOR", "NODE_MAJOR", "install_dropin", "build"]
 
 

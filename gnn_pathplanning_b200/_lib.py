@@ -14,7 +14,7 @@ import threading
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC_DIR = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libgnnpp_b200.so")
-SOURCES = ("graph_filter.cu", "graph_filter_tc.cu", "graph_filter_pair.cu", "graph_filter_small.cu", "rollout.cu", "feature.cu", "feature_tc.cu", "feature_mma.cu", "train.cu", "planner.cu", "expert_data.cu", "expert_solve.cu")
+SOURCES = ("graph_filter.cu", "graph_filter_tc.cu", "graph_filter_pair.cu", "graph_filter_small.cu", "rollout.cu", "feature.cu", "feature_tc.cu", "feature_mma.cu", "train.cu", "planner.cu", "expert_data.cu", "expert_solve.cu", "case_gen.cu")
 HEADERS = ("common.cuh", "feature.cuh", "tc_common.cuh", "rollout_common.cuh")
 INCLUDE = os.path.join(os.path.dirname(PKG_DIR), "include", "gnnpp_b200.h")
 INCLUDE_DEBUG = os.path.join(os.path.dirname(PKG_DIR), "include", "gnnpp_b200_debug.h")
@@ -43,7 +43,7 @@ EXPORTED = (
     "gpp_planner_forward", "gpp_planner_forward_host",
     "gpp_planner_train_workspace_bytes", "gpp_planner_train_forward", "gpp_planner_train_backward", "gpp_planner_ce_loss", "gpp_rollout_build_inputs", "gpp_rollout_move",
     "gpp_rollout_expert_metrics", "gpp_rollout_record", "gpp_expert_radius", "gpp_expert_gather",
-    "gpp_expert_solve_workspace_bytes", "gpp_expert_solve",
+    "gpp_expert_solve_workspace_bytes", "gpp_expert_solve", "gpp_case_generate",
     "gpp_planner_forward_host_async", "gpp_planner_wait", "gpp_planner_forward_async", "gpp_planner_join",
     "gpp_planner_set_profiling", "gpp_planner_get_profile",
     "gpp_planner_set_graph_filter_mode", "gpp_planner_set_feature_mode",
@@ -199,6 +199,8 @@ def load():
         lib.gpp_expert_solve_workspace_bytes.argtypes = [i, i, i, i, i]
         lib.gpp_expert_solve.restype = i
         lib.gpp_expert_solve.argtypes = [vp, vp, vp, i, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, i, i, i, vp]
+        lib.gpp_case_generate.restype = i
+        lib.gpp_case_generate.argtypes = [C.c_ulonglong, C.c_ulonglong, i, i, i, i, i, vp, vp, vp, vp, vp]
         lib.gpp_planner_forward_host_async.restype = i
         lib.gpp_planner_forward_host_async.argtypes = [vp, vp, vp, i, vp, i, i, C.POINTER(C.c_ulonglong)]
         lib.gpp_planner_wait.restype = i

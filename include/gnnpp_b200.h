@@ -365,6 +365,41 @@ int gpp_expert_solve(const unsigned char* map, const int* start, const int* goal
                      int* tau, short* paths, void* workspace, size_t workspace_bytes, int C, int N, int W,
                      void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * Expert case generation (replaces offlineExpert/CasesGenerator.py's mapGen, img_fill and setup_cases): K candidates
+ * per call, numbered first_candidate, first_candidate + 1, ...  A candidate is a W x W maze, its filled map and N
+ * (start, goal) pairs.  Its randomness is a pure function of (seed, k), so the result does not depend on the launch.
+ *
+ * Draws: Philox4x32-10, key (seed & 0xffffffff, seed >> 32), counter (k & 0xffffffff, k >> 32, block, phase); phase 0
+ *   is the maze, phase 1 the agents.  Draw j of a phase is word j % 4 of block j / 4.  A bounded draw in [0, n) is
+ *   (u32 * n) >> 32 in 64-bit arithmetic, no rejection.
+ * Maze (mapGen with height = width = W): all free; aisles times: col = 2 draw(W/2), then row = 2 draw(W/2), mark
+ *   (row, col); then walk steps, each building the neighbour list (row, col-2) if col > 1, (row, col+2) if col < W-2,
+ *   (row-2, col) if row > 1, (row+2, col) if row < W-2.  A non-empty list picks list[draw(len - 1)] (the last entry is
+ *   never picked); a free pick is marked with the cell between and becomes the position.  An empty list draws nothing.
+ *   aisles = int(density * ((W//2) * (W//2))) and walk = int(complexity * (5 * (W + W))) are the caller's.
+ * Fill (img_fill): the free cells are the 4-connected free component of the maze containing (0, 0); every other cell
+ *   is an obstacle.  If (0, 0) is an obstacle there are no free cells.
+ * Agents (random.sample(free cells, 2) per agent): F free cells in row-major order; agent i draws s = draw(F) (phase-1
+ *   word 2i) and g' = draw(F - 1) (word 2i + 1); goal index g = g' + (g' >= s).  Cells are (x, y) = (row, col).
+ * Status: GPP_CASE_TOO_FEW_FREE when F < 2, GPP_CASE_SHARED_CELL when two agents share a start or a goal,
+ *   GPP_CASE_ACCEPTED otherwise.
+ *
+ * All pointers are device pointers.  Envelope: 1 <= N <= 64, 2 <= W <= 64, aisles * (2 + walk) < 2^31, else
+ * GPP_ERR_UNSUPPORTED.
+ *   map [K,W,W] uint8 out: the filled map, 1 = obstacle
+ *   start, goal [K,N,2] int32 out: cells (x, y); -1 for a GPP_CASE_TOO_FEW_FREE candidate
+ *   status [K] int32 out (gpp_case_status)
+ * ---------------------------------------------------------------------------------- */
+typedef enum gpp_case_status {
+    GPP_CASE_ACCEPTED = 0,
+    GPP_CASE_TOO_FEW_FREE = 1,
+    GPP_CASE_SHARED_CELL = 2
+} gpp_case_status;
+
+int gpp_case_generate(unsigned long long seed, unsigned long long first_candidate, int K, int N, int W, int aisles,
+                      int walk, unsigned char* map, int* start, int* goal, int* status, void* stream);
+
 /* Asynchronous variant for pipelined rollouts over INDEPENDENT episode batches: stages the inputs on a copy stream,
  * enqueues the forward on one of the planner's four compute streams (tickets rotate over them, so the feature kernel of
  * one batch runs next to the kernels of the batches before it on the SMs they leave idle) and returns at once with a completion ticket; the
